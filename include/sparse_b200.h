@@ -287,6 +287,29 @@ int b2s_mttkrp(int dtype, int idx_bytes, int64_t I_, int64_t J, const void *indp
                const void *l_dev, const void *vals_dev, const void *d_dev, int64_t ldd, const void *c_dev, int64_t ldc,
                void *out_dev, int64_t ldo, void *stream);
 
+/* ---- mode-n MTTKRP of a sparse tensor of order 2..8 (K10, mttkrp.cu; no reference counterpart) ------------------
+ * out[i, r] = sum over stored entries e with i_mode(e) = i of v_e * prod_{m != mode} U_m[i_m(e), r], out dense
+ * (rows x R, row stride ldo), fully written.  coords_host[m] (m < order) are device pointers to the coordinate arrays
+ * of the MODE STREAM S_mode, vals_dev its values; factors_host[m] / ld_host[m] (row stride in elements) are the
+ * factor matrices, entry `mode` is never read (may be NULL).  No stream synchronisation.
+ *
+ * Fixed order of operations (results are reproducible bit for bit, whatever the grid, SM count or stream):
+ *  1. S_mode is the canonical (C-order) entry order for mode 0, and that order sorted stably by coordinate `mode`
+ *     for any other mode.
+ *  2. p_e[r] = (((v_e * U_a[i_a, r]) * U_b[i_b, r]) * ...) over the modes a < b < ... other than `mode`, each
+ *     product rounded separately; no FMA contraction.
+ *  3. S_mode is cut into consecutive chunks of B2S_MTTKRP_CHUNK entries (b2s_mttkrp_mode_chunk()).
+ *  4. The partial of row i in chunk c is ((+0 + p_1) + p_2) + ... over that row's entries in the chunk, in stream
+ *     order, each sum rounded.
+ *  5. out[i, r] = ((+0 + partial_c1) + partial_c2) + ... over the chunks touching row i, in chunk order; a row
+ *     without entries is +0.
+ */
+#define B2S_MTTKRP_CHUNK 512
+int b2s_mttkrp_mode_chunk(void); /* returns B2S_MTTKRP_CHUNK */
+int b2s_mttkrp_mode(int dtype, int idx_bytes, int order, int mode, int64_t nnz, int64_t rows, int64_t R,
+                    const void *const *coords_host, const void *vals_dev, const void *const *factors_host,
+                    const int64_t *ld_host, void *out_dev, int64_t ldo, void *stream);
+
 /* ---- copy-engine exchange of a row-sharded dense operand (peer.cu; SURVEY.md s8(e), no reference counterpart: the
  * reference is single-process) ------------------------------------------------------------------------------------
  * b2s_peer_alloc: cudaMalloc'ed (IPC-exportable) device buffer; b2s_peer_export writes its 64-byte CUDA IPC handle;

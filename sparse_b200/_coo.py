@@ -144,8 +144,12 @@ class COO(SparseArray):
             self._canonicalise(check_sort=not sorted, sum_dups=has_duplicates, prune=prune)
 
     # ---- construction helpers ------------------------------------------------------------------------
+    # mode streams of mttkrp_mode ({(mode, int32 indices): (coordinate rows, values)}); belong to the current contents
+    _mode_streams = None
+
     def _copy_from(self, other):
         SparseArray.__init__(self, other.shape, fill_value=None)
+        self._mode_streams = None
         self._coords_np, self._data_np = other._coords_np, other._data_np
         self._coords, self._data, self._keys = other._coords, other._data, other._keys
         self._idx_vis = other._idx_vis
@@ -395,6 +399,7 @@ class COO(SparseArray):
                 keys = Kn.compact(keys, flags, pos, total)
                 changed = True
         if changed:
+            self._mode_streams = None
             idt = D.np_dtype(coords)
             # keep the caller's index dtype when it is not int64; otherwise derive coordinates lazily from the keys
             self._coords = Kn.unravel(keys, self.shape, idt) if idt != np.dtype(np.int64) else None

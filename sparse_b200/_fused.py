@@ -6,15 +6,21 @@
 The unfused expressions also run (through elemwise + reduce); these entry points avoid the dense (a @ b)
 intermediate and the nnz x J broadcast products.  Floating-point association differs from the reference's
 BLAS / reduceat order, so parity is tolerance-based (rtol 1e-5 f32, 1e-12 f64 in the tests).
+
+mttkrp_mode(X, factors, mode) generalises mttkrp to any mode of a tensor of order 2..8 (the CP-ALS step); it has no
+counterpart in the reference beyond the unfused broadcast expression / einsum.
 """
 from __future__ import annotations
 
+import operator
+
 import numpy as np
+from numpy.exceptions import AxisError
 
 from . import _device as D
 from . import _kernels as Kn
 from ._coo import COO
-from ._dot import _coo_as_csr, _dense_dev, _narrow_idx
+from ._dot import _coo_as_csr, _dense_dev, _narrow_idx, _return_dense
 from ._sparse_array import SparseArray
 from ._utils import check_zero_fill_value
 
@@ -89,3 +95,89 @@ def mttkrp(B, Dm, Cm):
     t = D.torch()
     res = COO._from_device(t.stack([rows, cols]), vals, (I_, J), T.type(0))
     return GCXS.from_coo(res) if was_gcxs else res
+
+
+# Test hook: True keeps the mode streams' coordinates int64 even when every extent and nnz fit int32.
+_FORCE_WIDE_INDEX = False
+
+
+def _mode_stream(X, mode):
+    """Coordinate rows (a list of N device index tensors) and values of X's entries in the order of the mode stream
+    S_mode: C order for mode 0, C order sorted stably by coordinate `mode` otherwise.  Cached on X per mode."""
+    from ._gcxs import GCXS
+    from ._utils import key_bits
+
+    limit = 2**63 if _FORCE_WIDE_INDEX else max(*X.shape, X.nnz)
+    key = (mode, limit < 2**31 - 1)
+    cache = X._mode_streams
+    if cache is not None and key in cache:
+        return cache[key]
+    c = X.tocoo() if isinstance(X, GCXS) else X
+    coords, vals = c._dev()
+    rows = [coords[m].contiguous() for m in range(X.ndim)]
+    if mode != 0:
+        sorted_rows, perm = Kn.sort_keys(Kn.cast(rows[mode], np.int64), key_bits(X.shape[mode]))
+        rows = [sorted_rows if m == mode else Kn.gather(rows[m], perm) for m in range(X.ndim)]
+        vals = Kn.gather(vals, perm)
+    stream = (_narrow_idx(*rows, limit=limit), vals)
+    if cache is None:
+        cache = X._mode_streams = {}
+    cache[key] = stream
+    return stream
+
+
+def mttkrp_mode(X, factors, mode):
+    """Mode-`mode` MTTKRP of a sparse tensor: the product of the mode-`mode` matricisation of `X` with the Khatri-Rao
+    product of every other factor, the step CP-ALS runs once per mode and iteration.
+
+        out[i, r] = sum over stored entries e with i_mode(e) = i of  v_e * prod_{m != mode} factors[m][i_m(e), r]
+
+    `X` is a COO or GCXS of order 2..8 with a zero fill value.  `factors` holds N dense 2-D arrays (NumPy arrays or
+    CUDA tensors), `factors[m]` of shape (X.shape[m], R) with one R for all; `factors[mode]` is never read and may be
+    None.  `mode` counts from the end when negative.  The result is dense, (X.shape[mode], R), of dtype
+    result_type(X.dtype, other factor dtypes) (float32 or float64): a NumPy array, or a CUDA tensor when a factor is
+    one.
+
+    The summation order is fixed (include/sparse_b200.h, b2s_mttkrp_mode), so results are reproducible bit for bit.
+    Product association differs from `mttkrp`, so the two agree to rounding, not bit for bit.
+
+    Memory: the entries ordered by coordinate `mode` are cached on `X` for the next call with the same mode (they are
+    dropped when X's contents are replaced, and are not copied or pickled).  A cached mode holds
+    (N * index bytes + value bytes) * nnz of device memory -- index bytes 4 when every extent and nnz fit int32, else 8.
+    """
+    from ._gcxs import GCXS
+
+    if not isinstance(X, (COO, GCXS)):
+        raise TypeError("mttkrp_mode: `X` must be a sparse_b200 COO or GCXS array")
+    N = X.ndim
+    if not 2 <= N <= 8:
+        raise ValueError(f"mttkrp_mode: order {N} outside 2..8")
+    check_zero_fill_value(X)
+    mode = operator.index(mode)
+    if not -N <= mode < N:
+        raise AxisError(mode, N)
+    mode %= N
+    factors = list(factors)
+    if len(factors) != N:
+        raise ValueError(f"mttkrp_mode: {len(factors)} factors for an order-{N} tensor")
+    others = [m for m in range(N) if m != mode]
+    for m in others:
+        if not D.is_device_tensor(factors[m]):
+            factors[m] = np.asarray(factors[m])
+    R = int(factors[others[0]].shape[1]) if factors[others[0]].ndim == 2 else -1
+    for m in others:
+        f = factors[m]
+        if f.ndim != 2 or int(f.shape[0]) != X.shape[m] or int(f.shape[1]) != R:
+            raise ValueError(f"mttkrp_mode: shape mismatch X{X.shape}, factor {m} {tuple(f.shape)} "
+                             f"(expected ({X.shape[m]}, R) with one R for all factors)")
+    T = np.result_type(X.dtype, *(_dense_dt(factors[m]) for m in others))
+    if T not in (np.dtype("float32"), np.dtype("float64")):
+        raise TypeError(f"mttkrp_mode: dtype {T} is outside the CUDA dtype matrix (float32, float64)")
+    rows = X.shape[mode]
+    if X.nnz == 0 or rows == 0 or R == 0:
+        out = Kn.full(rows * R, 0, T).reshape(rows, R)
+    else:
+        coords, vals = _mode_stream(X, mode)
+        fac = [None if m == mode else _dense_dev(factors[m], T) for m in range(N)]
+        out = Kn.mttkrp_mode(coords, Kn.cast(vals, T), fac, mode, rows, R)
+    return _return_dense(out, [f for f in factors if f is not None])

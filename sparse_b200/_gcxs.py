@@ -70,8 +70,12 @@ class GCXS(SparseArray):
         if prune:
             self._prune()
 
+    # mode streams of mttkrp_mode ({(mode, int32 indices): (coordinate rows, values)}); belong to the current contents
+    _mode_streams = None
+
     def _adopt(self, o):
         SparseArray.__init__(self, o.shape, fill_value=None)
+        self._mode_streams = None
         self._data_np, self._indices_np, self._indptr_np = o._data_np, o._indices_np, o._indptr_np
         self._data, self._indices, self._indptr = o._data, o._indices, o._indptr
         self._idx_vis = o._idx_vis
@@ -496,6 +500,7 @@ class GCXS(SparseArray):
         pos, total = Kn.scan_flags(flags)
         if total == self.nnz:
             return
+        self._mode_streams = None
         self._data = Kn.compact(data, flags, pos, total)
         self._indices = Kn.compact(indices, flags, pos, total)
         if self.ndim > 1:

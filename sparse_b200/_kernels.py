@@ -641,3 +641,41 @@ def mttkrp(indptr, kk, ll, vals, Dm, Cm, I_, J):
                                i64(J), vp(D.ptr(out)), i64(J), _sp())
     _lib.check(rc, "b2s_mttkrp")
     return out
+
+
+# ------------------------------------------------------------------------------------------------
+# K10 mode-n MTTKRP
+# ------------------------------------------------------------------------------------------------
+def mttkrp_mode_chunk() -> int:
+    """Entries per chunk of the mode stream (step 3 of the order in include/sparse_b200.h)."""
+    return int(_lib.load().b2s_mttkrp_mode_chunk())
+
+
+def mttkrp_mode(coords, vals, factors, mode, rows, R):
+    """out[i, r] = sum over the stream entries e with coords[mode][e] = i of vals[e] * prod_{m != mode}
+    factors[m][coords[m][e], r], in the fixed order of b2s_mttkrp_mode.  `coords` (N index tensors, one width) and
+    `vals` are the mode stream; factors[mode] is not read."""
+    t = _t()
+    N = len(coords)
+    dt = D.np_dtype(vals)
+    assert all(c.dtype == coords[0].dtype for c in coords)
+    fac, ld, keep = [], [], []
+    for m, f in enumerate(factors):
+        if m == mode:
+            fac.append(0)
+            ld.append(R)
+            continue
+        assert f.dtype == vals.dtype
+        if R > 1 and f.stride(1) != 1:
+            f = f.contiguous()
+        keep.append(f)  # a contiguous copy lives until the launch is enqueued (the caching allocator orders its reuse)
+        fac.append(D.ptr(f))
+        ld.append(f.stride(0) if f.shape[0] > 1 else R)
+    out = t.empty((rows, R), dtype=vals.dtype, device=vals.device)
+    ptrs = (ctypes.c_void_p * N)(*[D.ptr(c) for c in coords])
+    fptrs = (ctypes.c_void_p * N)(*fac)
+    rc = _lib.load().b2s_mttkrp_mode(i32(D.dtype_code(dt)), i32(_idx_bytes(coords[0])), i32(N), i32(mode),
+                                     i64(vals.shape[0]), i64(rows), i64(R), ptrs, vp(D.ptr(vals)), fptrs, _i64arr(ld),
+                                     vp(D.ptr(out)), i64(R), _sp())
+    _lib.check(rc, "b2s_mttkrp_mode")
+    return out

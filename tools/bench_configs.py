@@ -5,7 +5,7 @@ Device-resident inputs (generated with seeded torch generators on the GPU), wall
 torch.cuda.synchronize() because the public calls contain their own size-returning syncs.
 Prints one line per config as it runs and the whole result as one JSON line at the end.
 
-    python tools/bench_configs.py [c1 c3 c3big red c4 c5 mttkrp]
+    python tools/bench_configs.py [c1 c3 c3big red c4 c5 mttkrp mttkrp_mode]
 """
 import json
 import os
@@ -63,7 +63,7 @@ def run(which=None, compact=False, parity=True):
     sys.path.insert(0, os.path.join(ROOT, "tests", "golden"))
     import fullsize_inputs as FI
 
-    which = which or ["c1", "c3", "red", "c5", "c4", "mttkrp", "c3big"]
+    which = which or ["c1", "c3", "red", "c5", "c4", "mttkrp", "mttkrp_mode", "c3big"]
     res = {}
     _lib.load()
 
@@ -253,8 +253,84 @@ def run(which=None, compact=False, parity=True):
             r["parity"] = {"vs": "fp64 restatement sum_kl B[i,k,l] D[l,j] C[k,j], rtol 2e-5",
                            "values_close": bool(torch.allclose(got.double(), wantm, rtol=2e-5, atol=1e-9))}
             del contrib, wantm
+
+    if "mttkrp_mode" in which:
+        # K9's config, mode 0, next to the fused mttkrp above (same seeds)
+        I_, K_, L_, J = 10_000, 10_000, 1_000, 32
+        Bt = rand_coo((I_, K_, L_), 10_000_000, 31, torch.float32)
+        g = torch.Generator(device=DEV).manual_seed(32)
+        Dm = torch.rand((L_, J), generator=g, device=DEV, dtype=torch.float32)
+        Cm = torch.rand((K_, J), generator=g, device=DEV, dtype=torch.float32)
+        alg = Bt.nnz * (3 * 4 + 4) + Bt.nnz * 2 * J * 4 + I_ * J * 4
+        r = rec("MTTKRP mttkrp_mode mode 0 (1e4 x 1e4 x 1e3, nnz 1e7, J=32 f32)",
+                lambda: sp.mttkrp_mode(Bt, [None, Cm, Dm], 0), Bt.nnz, "Gnnz_s", alg)
+        if parity:
+            got = sp.mttkrp_mode(Bt, [None, Cm, Dm], 0)
+            co, dv = Bt._dev()
+            contrib = dv.double()[:, None] * Cm[co[1]].double() * Dm[co[2]].double()
+            wantm = torch.zeros((I_, J), dtype=torch.float64, device=DEV).index_add_(0, co[0], contrib)
+            r["parity"] = {"vs": "fp64 restatement sum_kl B[i,k,l] C[k,j] D[l,j], rtol 2e-5",
+                           "values_close": bool(torch.allclose(got.double(), wantm, rtol=2e-5, atol=0))}
+            del contrib, wantm
+        del Bt, Dm, Cm
+        res.update(_mttkrp_mode_order3(rec, parity))
     torch.cuda.empty_cache()
     return res
+
+
+def _mttkrp_mode_order3(rec, parity):
+    """CP-ALS workload: (1e6, 1e6, 100) with 1e8 uniform entries, R = 32, f32, factors on the device.  Modes 0 and 1
+    have ~100 entries per slice, mode 2 has 100 slices of ~1e6 entries (the skewed case)."""
+    sys.path.insert(0, os.path.join(ROOT, "tests"))
+    import _mttkrp_order as MO
+
+    shape, R = (1_000_000, 1_000_000, 100), 32
+    X = rand_coo(shape, 100_000_000, 41, torch.float32)
+    g = torch.Generator(device=DEV).manual_seed(42)
+    U = [torch.rand((s, R), generator=g, device=DEV, dtype=torch.float32) for s in shape]
+    coords, vals = X._dev()
+    nnz, N, ib, vb = X.nnz, 3, 4, 4
+    ch = sp._kernels.mttkrp_mode_chunk()
+    out = {}
+    for mode in range(N):
+        X._mode_streams = None  # first call: builds the mode stream (sort + gathers + narrowing)
+        torch.cuda.synchronize()
+        t0 = time.perf_counter()
+        sp.mttkrp_mode(X, U, mode)
+        torch.cuda.synchronize()
+        first = (time.perf_counter() - t0) * 1e3
+        alg = nnz * (N * ib + vb) + nnz * (N - 1) * R * vb + shape[mode] * R * vb
+        name = f"mttkrp_mode order-3 (1e6,1e6,100) nnz 1e8 R=32 f32 mode {mode}"
+        r = rec(name, lambda: sp.mttkrp_mode(X, U, mode), nnz, "Gnnz_s", alg)
+        r["first_call_ms"] = round(first, 3)
+        r["gather_model_bytes"] = int(alg)
+        if parity:
+            got = sp.mttkrp_mode(X, U, mode)
+            want = torch.zeros((shape[mode], R), dtype=torch.float64, device=DEV)
+            for s in range(0, nnz, 10_000_000):
+                c = coords[:, s:s + 10_000_000]
+                p = vals[s:s + 10_000_000].double()[:, None]
+                for m in range(N):
+                    if m != mode:
+                        p = p * U[m][c[m]].double()
+                want.index_add_(0, c[mode], p)
+            close = bool(torch.allclose(got.double(), want, rtol=2e-5, atol=0))
+            del want
+            rows = np.random.default_rng(mode).choice(shape[mode], 4, replace=False)
+            exact = True
+            for i in rows:
+                sel = torch.nonzero(coords[mode] == int(i)).reshape(-1)
+                start = int((coords[mode] < int(i)).sum())
+                c = coords[:, sel]
+                p = MO.products(vals[sel].cpu().numpy(), [U[m][c[m]].cpu().numpy() for m in range(N) if m != mode],
+                                np.float32)
+                exact &= MO.same_bits(got[int(i)].cpu().numpy(), MO.row_result(p, start, ch, np.float32))
+            r["parity"] = {"vs": "fp64 device restatement (all rows, rtol 2e-5) + 4 sampled rows bit-compared with "
+                                 "the CPU restatement of the order (tests/_mttkrp_order.py)",
+                           "values_close": close, "sampled_rows_bit_exact": bool(exact)}
+        out[name] = r
+    del X, U, coords, vals
+    return out
 
 
 def main():
