@@ -103,13 +103,19 @@ int b2s_spmm_host_set_pipeline(int chunks, int slots);
 /* The host-side narrowing step on its own (same thread pool): dst[i] = (int32) src[i]. */
 int b2s_host_narrow_i64_i32(const int64_t *src_host, int32_t *dst_host, int64_t n);
 
-/* 1 if every row of the CSR has non-decreasing column indices (precondition of the panel passes). Synchronises. */
+/* 1 if every row of the CSR has non-decreasing column indices. Synchronises. */
 int b2s_csr_rows_sorted(int idx_bytes, int64_t M, const void *indptr_dev, const void *indices_dev, int *sorted_host,
                         void *stream);
 /*
- * K1 with explicit scheduling: n_panels <= 1 -> the one-pass kernel; n_panels >= 2 -> column-panel passes that keep
- * the active slice of B resident in L2 (rows must be sorted by column: rows_sorted = 1; bit-identical results);
- * n_panels == 0 -> choose from the size of B (~48 MB per panel) and nnz / M.  nnz < 0 = unknown.
+ * K1 with explicit scheduling: n_panels == 1 -> the one-pass kernel; n_panels >= 2 -> tiled passes (one per column
+ * tile x K panel, with n_panels K panels) that serve the B-row gathers from L2; n_panels == 0 -> tiled passes when B
+ * is larger than twice the L2, nnz >= 64 K and the dtype is fp32 (panel count from the panel budget), the one-pass
+ * kernel otherwise.
+ * The tiled passes need fp32/fp64 and 16-byte aligned operands (N, ldb, ldc multiples of 16 bytes); other calls take
+ * the one-pass kernel.  Rows must be sorted by column for the passes: a device-side check sends a call with any
+ * unsorted row to the one-pass kernel, without a host synchronisation.  rows_sorted is advisory (0 = known unsorted,
+ * skip the passes; 1 or -1 = sorted or unknown).  long_rows selects the nnz-balanced long-row path (one-pass kernel).
+ * Results are bit-identical on every path.  nnz < 0 = unknown (automatic choice: one-pass kernel).
  */
 int b2s_spmm_csr_dense_ex(int dtype, int idx_bytes, int64_t M, int64_t K, int64_t N, int64_t nnz,
                           const void *a_data_dev, const void *a_indices_dev, const void *a_indptr_dev,
@@ -122,8 +128,13 @@ int b2s_csr_max_row_nnz(int idx_bytes, int64_t M, const void *indptr_dev, int64_
 
 /* Tuning knob for K1 (0 = default).  variant: 1 = register-staged LDG gather with DYNAMIC row assignment (persistent
  * warps draw rows from a counter; the default), 3 = the same gather on the static one-row-per-warp grid,
- * 2 = 1-D bulk-TMA (cp.async.bulk) gather through a shared-memory ring. */
+ * 2 = 1-D bulk-TMA (cp.async.bulk) gather through a shared-memory ring, 4 = the default one-pass kernel, with the
+ * tiled passes loading B without the L2 evict_last policy. */
 int b2s_spmm_set_variant(int variant, int unroll);
+/* Tuning of the tiled passes of b2s_spmm_csr_dense_ex (process-wide; 0 = default): panel_bytes = bytes of B (one K
+ * panel x one column tile) per pass, which sets the panel count of the automatic choice (default 24 MB);
+ * tile_bytes = width of a column tile, 64, 128 (default: one cache line) or 256. */
+int b2s_spmm_set_tiling(int64_t panel_bytes, int tile_bytes);
 /* process-wide default of the nnz-balanced long-row path used by b2s_spmm_csr_dense (default off; b2s_spmm_csr_dense_ex
  * selects it per call; results stay bit-identical). */
 int b2s_spmm_set_skew(int enabled);

@@ -59,14 +59,16 @@ def empty(n, dtype, like=None):
 # ------------------------------------------------------------------------------------------------
 # K1
 # ------------------------------------------------------------------------------------------------
-def spmm_csr_dense(a_data, a_indices, a_indptr, b, M: int, K: int, N: int, out=None, *, n_panels=1,
+def spmm_csr_dense(a_data, a_indices, a_indptr, b, M: int, K: int, N: int, out=None, *, n_panels=0,
                    rows_sorted=None, long_rows=False):
     """out[M,N] = CSR(A) @ B -- replaces _dot_csr_ndarray (_common.py:720-755).
 
     All arguments are CUDA tensors; `b` is (K, N) row-major (row stride may exceed N).
     Bit-identical to the reference loop (stored order, unfused multiply/add).
-    n_panels: 1 = one-pass kernel; >= 2 = column-panel passes (L2-resident slices of B; needs rows sorted by
-    column); 0 = let the library choose from the size of B and nnz / M.
+    n_panels: 0 = let the library choose from the size of B and nnz / K; 1 = one-pass kernel; >= 2 = tiled passes
+    with that many K panels (B-row gathers served from L2).  The passes check on the device that rows are sorted by
+    column and leave the call to the one-pass kernel otherwise, with no host synchronisation.  rows_sorted is a hint:
+    False skips the passes.
     """
     lib = _lib.load()
     t = _t()
@@ -79,12 +81,10 @@ def spmm_csr_dense(a_data, a_indices, a_indptr, b, M: int, K: int, N: int, out=N
         out = t.empty((M, N), dtype=a_data.dtype, device=a_data.device)
     ldb = b.stride(0) if K > 1 else max(N, 1)
     ldc = out.stride(0) if M > 1 else max(N, 1)
-    if n_panels != 1 and rows_sorted is None:
-        rows_sorted = csr_rows_sorted(a_indices, a_indptr, M)
     rc = lib.b2s_spmm_csr_dense_ex(
         i32(D.dtype_code(dt)), i32(_idx_bytes(a_indices)), i64(M), i64(K), i64(N), i64(a_data.shape[0]),
         vp(D.ptr(a_data)), vp(D.ptr(a_indices)), vp(D.ptr(a_indptr)), vp(D.ptr(b)), i64(max(ldb, N)), vp(D.ptr(out)),
-        i64(max(ldc, N)), i32(n_panels if (n_panels == 1 or rows_sorted) else 1), i32(1 if rows_sorted else 0),
+        i64(max(ldc, N)), i32(n_panels), i32(-1 if rows_sorted is None else (1 if rows_sorted else 0)),
         i32(1 if long_rows else 0), _sp(),
     )
     _lib.check(rc, "b2s_spmm_csr_dense_ex")
@@ -133,6 +133,11 @@ def spmm_csr_dense_host(a_data: np.ndarray, a_indices: np.ndarray, a_indptr: np.
 
 def spmm_set_variant(variant: int = 1, unroll: int = 8):
     _lib.check(_lib.load().b2s_spmm_set_variant(i32(variant), i32(unroll)))
+
+
+def spmm_set_tiling(panel_bytes: int = 0, tile_bytes: int = 0):
+    """Tiled passes of spmm_csr_dense (process-wide, 0 = default): B bytes per pass, column-tile width (64/128/256)."""
+    _lib.check(_lib.load().b2s_spmm_set_tiling(i64(panel_bytes), i32(tile_bytes)))
 
 
 def spmm_host_set_threads(n: int = -1):

@@ -69,6 +69,9 @@ int spmm_csr_dense_impl(int dtype, int idx_bytes, int64_t M, int64_t K, int64_t 
                         const void *ap, const void *b, int64_t ldb, void *out, int64_t ldc, cudaStream_t s);
 int narrow_i64_i32(const int64_t *in, int32_t *out, int64_t n, cudaStream_t s);
 void set_call_skew(int v);  // per-call override of the long-row path (-1 = process default)
+// per-call guard of the one-pass kernel: it returns at entry while *guard == 0 (nullptr = always runs)
+void set_call_guard(const int *guard);
+extern int g_tile_hint;  // spmm_panel.cu: L2 evict_last hint on the B loads of the tiled passes (tuning)
 
 // ---------------------------------------------------------------------------
 // exact (non-contracted) arithmetic: the reference rounds a*b and (+) separately

@@ -53,9 +53,10 @@ template <typename T, typename I, int VEC, int G, int U>
 __global__ void __launch_bounds__(256)
 spmm_csr_dense_kernel(int64_t M, int64_t N, const T *__restrict__ a_data, const I *__restrict__ a_indices,
                       const I *__restrict__ a_indptr, const T *__restrict__ B, int64_t ldb, T *__restrict__ C,
-                      int64_t ldc, const uint8_t *__restrict__ skip) {
+                      int64_t ldc, const uint8_t *__restrict__ skip, const int *__restrict__ guard) {
     static_assert(G >= 1 && G <= 32 && (G & (G - 1)) == 0, "G must be a power of two <= 32");
     static_assert(U <= G && G % U == 0, "U must divide G");
+    if (guard != nullptr && *guard == 0) return;  // the tiled passes (spmm_panel.cu) computed this call
     constexpr unsigned FULL = 0xffffffffu;
     constexpr int ROWS_PER_WARP = 32 / G;
     const int lane = threadIdx.x & 31;
@@ -130,9 +131,11 @@ template <typename T, typename I, int VEC, int G, int U, int MINB>
 __global__ void __launch_bounds__(256, MINB)
 spmm_csr_dense_dyn_kernel(int64_t M, int64_t N, const T *__restrict__ a_data, const I *__restrict__ a_indices,
                       const I *__restrict__ a_indptr, const T *__restrict__ B, int64_t ldb, T *__restrict__ C,
-                      int64_t ldc, const uint8_t *__restrict__ skip, unsigned int *__restrict__ row_counter) {
+                      int64_t ldc, const uint8_t *__restrict__ skip, unsigned int *__restrict__ row_counter,
+                      const int *__restrict__ guard) {
     static_assert(G >= 1 && G <= 32 && (G & (G - 1)) == 0, "G must be a power of two <= 32");
     static_assert(U <= G && G % U == 0, "U must divide G");
+    if (guard != nullptr && *guard == 0) return;  // the tiled passes (spmm_panel.cu) computed this call
     constexpr unsigned FULL = 0xffffffffu;
     constexpr int ROWS_PER_WARP = 32 / G;
     const int lane = threadIdx.x & 31;
@@ -342,6 +345,8 @@ static int g_dyn_form = 0;     // tuning of the dynamic-row kernel (see dispatch
 static int g_static_rows = 0;  // 1 = the static one-row-per-warp grid instead of the dynamic-row default (A/B, tests)
 static thread_local int t_skew = -1;
 void set_call_skew(int v) { t_skew = v; }
+static thread_local const int *t_guard = nullptr;
+void set_call_guard(const int *guard) { t_guard = guard; }
 
 // spmm_skew.cu
 template <typename T, typename I>
@@ -361,7 +366,7 @@ static int launch_v1(int64_t M, int64_t N, const void *ad, const void *ai, const
                 (long long)M, (long long)N);
     dim3 grid((unsigned)gx, (unsigned)gy);
     spmm_csr_dense_kernel<T, I, VEC, G, U><<<grid, THREADS, 0, s>>>(M, N, (const T *)ad, (const I *)ai, (const I *)ap,
-                                                                    (const T *)b, ldb, (T *)out, ldc, skip);
+                                                                    (const T *)b, ldb, (T *)out, ldc, skip, t_guard);
     B2S_CHECK_LAUNCH();
     return B2S_OK;
 }
@@ -399,7 +404,7 @@ static int dispatch_g(int64_t M, int64_t N, const void *ad, const void *ai, cons
             // 2 = 8 in flight, 5 CTAs per SM; 3 = 16 in flight, 3 CTAs per SM.  H100 SXM at C2: 16.19 / 23.65 / 17.80 /
             // 18.36 ms (tools/tune_k1_dyn.py)
             using KernT = void (*)(int64_t, int64_t, const T *, const I *, const I *, const T *, int64_t, T *, int64_t,
-                                   const uint8_t *, unsigned int *);
+                                   const uint8_t *, unsigned int *, const int *);
             KernT kern = spmm_csr_dense_dyn_kernel<T, I, VEC, 32, 8, 4>;
             if (g_dyn_form == 1) kern = spmm_csr_dense_dyn_kernel<T, I, VEC, 32, 16, 4>;
             else if (g_dyn_form == 2) kern = spmm_csr_dense_dyn_kernel<T, I, VEC, 32, 8, 5>;
@@ -412,7 +417,7 @@ static int dispatch_g(int64_t M, int64_t N, const void *ad, const void *ai, cons
             if (blocks > need) blocks = need > 0 ? need : 1;
             dim3 grid((unsigned)blocks, (unsigned)gy);
             kern<<<grid, 256, 0, s>>>(M, N, (const T *)ad, (const I *)ai, (const I *)ap, (const T *)b, ldb, (T *)out, ldc,
-                                      skip, counter);
+                                      skip, counter, t_guard);
             B2S_CHECK_LAUNCH();
             if (own) scratch_free(own, s);
             return skew ? skew_end(s, skip) : B2S_OK;
@@ -510,6 +515,7 @@ int b2s_spmm_set_variant(int variant, int unroll) {
     g_static_rows = (variant == 3) ? 1 : 0;
     g_dyn_form = (variant >= 10 && variant <= 13) ? variant - 10 : 0;  // 10..13: forms of the dynamic-row kernel
     g_unroll = (unroll == 4 || unroll == 16 || unroll == 32) ? unroll : 8;
+    g_tile_hint = (variant == 4) ? 0 : 1;  // 4: tiled passes load B with no L2 policy (evict_last A/B)
     return B2S_OK;
 }
 

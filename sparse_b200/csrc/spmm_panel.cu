@@ -1,14 +1,19 @@
-// spmm_panel.cu -- K1p: CSR x dense with COLUMN-PANEL passes that keep the active slice of B resident in L2.
+// spmm_panel.cu -- K1p: CSR x dense in (column tile x K panel) passes that serve the B-row gathers from L2.
 //
-// Same contract as K1 (bit-identical to _dot_csr_ndarray, sparse/numba_backend/_common.py:720-755).  At C2 the
-// one-pass kernel is DRAM-bound: B (512 MB) cannot live in the 50 MB L2, so most of the 512-byte row gathers go to
-// HBM.  Here the K axis is cut into P panels of B rows small enough to stay in L2; pass p processes,
-// for every row of A, only the stored entries whose column falls into panel p.  Rows are sorted by column, so these
-// are a contiguous run that starts where pass p-1 stopped (a per-row cursor), and the partial sums are carried
-// through C in fp32 -- a store followed by a load of the same float is exact, and panels are visited in ascending
-// column order, so every out[i,j] still sees the reference's operation sequence.
-// DRAM traffic becomes  B once + A ~once + C (2P-1) x; the gathers are served by L2.
-// B rows carry an evict_last policy, the A stream, the cursor and the C read-modify-write are streaming accesses.
+// Same contract as K1 (bit-identical to _dot_csr_ndarray, sparse/numba_backend/_common.py:720-755).  At C2 (B is
+// 1e6 x 128 fp32 = 512 MB, L2 is 50 MB) the one-pass kernel gathers one 512-byte row of B per stored entry and almost
+// every gather misses L2: ~50 GB of HBM traffic for ~1.8 GB of compulsory bytes.  Here B is cut both ways:
+//   * a column tile of TB bytes (default 128 B = one cache line: 32 fp32 / 16 fp64 columns), and
+//   * P panels of the K axis (rows of B), so that one panel x one tile of B (K/P x TB bytes) fits in L2.
+// One launch per (tile, panel), tiles outer, panels inner.  Pass (t, p) computes, for every row of A, the stored entries
+// whose column falls into panel p, for the columns of tile t.  Rows are sorted by column, so these form the run
+// [off[p][row], off[p+1][row]) that a pre-pass computes once per call.  Partial sums are carried through C in T: a store
+// followed by a load of the same float is exact, panels are visited in ascending column order, and each run is taken
+// in stored order, so every out[i,j] is still ((+0 + a0*b0) + a1*b1) + ... with separate roundings, as in K1.
+// DRAM traffic: B once, A once per tile, C (2P-1) x per tile (reads and writes of one tile's columns).
+//
+// Any row with a descending column pair sets a device flag in the pre-pass; the passes then return at entry and the
+// one-pass kernel, launched behind them with the same flag as its guard, computes the whole product.  No host sync.
 #include "common.cuh"
 
 namespace b2s {
@@ -24,90 +29,161 @@ __device__ __forceinline__ uint4 ldg_cs_v4(const void *p) {
     return r;
 }
 
-template <typename T, typename I, int U>
+__device__ __forceinline__ uint64_t policy_evict_normal() {
+    uint64_t p;
+    asm volatile("createpolicy.fractional.L2::evict_normal.b64 %0, 1.0;" : "=l"(p));
+    return p;
+}
+
+// Pre-pass: one warp per row.  off is panel-major, (P+1) x M: off[p*M + row] = first position of the row whose column is
+// in panel >= p (off[0] = indptr[row], off[P] = indptr[row+1]).  Each lane handles one position j and writes off[p] = j
+// for the panels p in (panel(j-1), panel(j)]; the position j = end closes the row with panel P.  A sorted row therefore
+// writes each of its P+1 offsets exactly once.  *unsorted |= 1 if a row has a descending neighbour pair.
+template <typename I>
 __global__ void __launch_bounds__(256)
-spmm_panel_kernel(int64_t M, int64_t N, const T *__restrict__ a_data, const I *__restrict__ a_indices,
-                  const I *__restrict__ a_indptr, const I *__restrict__ cursor_in, I *__restrict__ cursor_out,
-                  const T *__restrict__ B, int64_t ldb,
-                  T *__restrict__ C, int64_t ldc, int64_t col_hi, int first, int last) {
-    constexpr int VEC = 16 / sizeof(T);
+panel_offsets_kernel(int64_t M, const I *__restrict__ indptr, const I *__restrict__ indices, int64_t width, int P,
+                     I *__restrict__ off, int *__restrict__ unsorted) {
     constexpr unsigned FULL = 0xffffffffu;
     const int lane = threadIdx.x & 31;
-    const int64_t row = (int64_t)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
-    if (row >= M) return;
-    const int64_t col0 = ((int64_t)blockIdx.y * 32 + lane) * VEC;
-    const bool col_ok = col0 < N;
-    int64_t base = first ? (int64_t)a_indptr[row] : (int64_t)cursor_in[row];
-    const int64_t end = (int64_t)a_indptr[row + 1];
-    const uint64_t pol_b = policy_evict_last();
-    const T *bcol = B + col0;
-    T *crow = C + row * ldc + col0;
-
-    PPack<T, VEC> acc;
-#pragma unroll
-    for (int k = 0; k < VEC; ++k) acc.v[k] = T(0);
-    // nothing of this row in this panel (and not the initialising pass): leave C and the cursor untouched
-    I col = 0;
-    T val = T(0);
-    int cnt = 0;
-    {
-        const int64_t rem = end - base;
-        cnt = rem > 32 ? 32 : (rem > 0 ? (int)rem : 0);
-        if (lane < cnt) {
-            col = ldg_stream(a_indices + base + lane);
-            val = ldg_stream(a_data + base + lane);
+    const int64_t nwarps = ((int64_t)gridDim.x * blockDim.x) >> 5;
+    bool bad = false;
+    for (int64_t row = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5; row < M; row += nwarps) {
+        const int64_t s = (int64_t)ldg_stream(indptr + row), e = (int64_t)ldg_stream(indptr + row + 1);
+        if (lane == 0) __stcs(off + row, (I)s);
+        I carry_c = 0;
+        int carry_q = 0;
+        for (int64_t j0 = s; j0 <= e; j0 += 32) {
+            const int64_t j = j0 + lane;
+            const bool valid = j < e;
+            I c = 0;
+            int q = P;  // positions at or past the end close the row
+            if (valid) {
+                c = ldg_stream(indices + j);
+                bad |= c < 0;
+                int64_t qq;
+                if constexpr (sizeof(I) == 4) qq = width > 0xffffffffll ? 0 : (int64_t)((uint32_t)c / (uint32_t)width);
+                else qq = (int64_t)((uint64_t)c / (uint64_t)width);
+                q = qq < P - 1 ? (int)qq : P - 1;
+            }
+            I cp = __shfl_up_sync(FULL, c, 1);
+            int qp = __shfl_up_sync(FULL, q, 1);
+            if (lane == 0) {
+                cp = carry_c;
+                qp = carry_q;
+            }
+            if (valid && j > s && c < cp) bad = true;
+            if (j <= e)
+                for (int p = qp + 1; p <= q; ++p) __stcs(off + (int64_t)p * M + row, (I)j);
+            carry_c = __shfl_sync(FULL, c, 31);
+            carry_q = __shfl_sync(FULL, q, 31);
         }
     }
-    unsigned m = __ballot_sync(FULL, lane < cnt && (int64_t)col < col_hi);
-    int take = __popc(m);
-    if (take == 0 && !first) {
-        // column tiles of the same row read cursor_in concurrently: the cursor is double-buffered per pass
-        if (!last && blockIdx.y == 0 && lane == 0) cursor_out[row] = (I)base;
-        return;
+    if (__any_sync(FULL, bad) && lane == 0) atomicOr(unsorted, 1);
+}
+
+// One pass (column tile at col_base, K panel [off_lo, off_hi)).  A group of L lanes owns one row and one tile of L x 16
+// bytes; lane `sub` holds columns col_base + sub*VEC .. +VEC.  Each chunk of L stored entries puts L independent
+// 16-byte B loads in flight per lane (one full line per group at L = 8).  Persistent warps walk rows with a static
+// stride; the next row's first A chunk and the offsets of the row after it are loaded before the current row's gathers,
+// so the offsets -> A -> B -> C chain of a row overlaps the gathers of the previous one.
+template <typename T, typename I, int L>
+__global__ void __launch_bounds__(256)
+spmm_tile_pass_kernel(int64_t M, int64_t N, const T *__restrict__ a_data, const I *__restrict__ a_indices,
+                      const I *__restrict__ off_lo, const I *__restrict__ off_hi, const T *__restrict__ B, int64_t ldb,
+                      T *__restrict__ C, int64_t ldc, int64_t col_base, int first, int hint,
+                      const int *__restrict__ unsorted) {
+    if (*unsorted) return;  // the one-pass kernel behind the passes computes this call
+    constexpr int VEC = 16 / sizeof(T);
+    constexpr int RPW = 32 / L;  // rows per warp
+    constexpr unsigned FULL = 0xffffffffu;
+    const int lane = threadIdx.x & 31;
+    const int sub = lane & (L - 1);
+    const int grp = lane / L;
+    const int64_t col0 = col_base + (int64_t)sub * VEC;
+    const bool col_ok = col0 < N;
+    const int64_t warp0 = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
+    const int64_t nwarps = ((int64_t)gridDim.x * blockDim.x) >> 5;
+    const int64_t stride = nwarps * RPW;
+    const uint64_t pol_b = hint ? policy_evict_last() : policy_evict_normal();
+    const T *bcol = B + col0;
+
+    int64_t row = warp0 * RPW + grp;
+    int64_t s = 0, e = 0, sn = 0, en = 0;
+    if (row < M) {
+        s = (int64_t)ldg_stream(off_lo + row);
+        e = (int64_t)ldg_stream(off_hi + row);
     }
-    if (!first && col_ok) {
-        const uint4 u = ldg_cs_v4(crow);
-        memcpy(&acc, &u, 16);
+    if (row + stride < M) {
+        sn = (int64_t)ldg_stream(off_lo + row + stride);
+        en = (int64_t)ldg_stream(off_hi + row + stride);
     }
-    while (true) {
-#pragma unroll 1
-        for (int j = 0; j < take; j += U) {
-            PPack<T, VEC> bv[U];
+    I colv = 0;
+    T valv = T(0);
+    if (s + sub < e) {
+        colv = ldg_stream(a_indices + s + sub);
+        valv = ldg_stream(a_data + s + sub);
+    }
+    for (int64_t w = warp0; w * RPW < M; w += nwarps, row += stride) {
+        // prefetch: first A chunk of the next row, offsets of the row after it
+        I colv_n = 0;
+        T valv_n = T(0);
+        if (sn + sub < en) {
+            colv_n = ldg_stream(a_indices + sn + sub);
+            valv_n = ldg_stream(a_data + sn + sub);
+        }
+        int64_t s2 = 0, e2 = 0;
+        if (row + 2 * stride < M) {
+            s2 = (int64_t)ldg_stream(off_lo + row + 2 * stride);
+            e2 = (int64_t)ldg_stream(off_hi + row + 2 * stride);
+        }
+        const bool row_ok = row < M;
+        T *crow = C + row * ldc + col0;
+        PPack<T, VEC> acc;
 #pragma unroll
-            for (int u = 0; u < U; ++u) {
-                const I c = __shfl_sync(FULL, col, (j + u) & 31);
-                if (j + u < take && col_ok) {
+        for (int k = 0; k < VEC; ++k) acc.v[k] = T(0);
+        if (!first && s < e && col_ok) {
+            const uint4 u = ldg_cs_v4(crow);
+            memcpy(&acc, &u, 16);
+        }
+        for (int64_t base = s; __any_sync(FULL, base < e); base += L) {
+            const I col = colv;
+            const T val = valv;
+            const int64_t rem = e - base;
+            const int cnt = rem > L ? L : (rem > 0 ? (int)rem : 0);
+            if (base + L + sub < e) {  // next chunk of this row while this one is consumed
+                colv = ldg_stream(a_indices + base + L + sub);
+                valv = ldg_stream(a_data + base + L + sub);
+            }
+            PPack<T, VEC> bv[L];
+#pragma unroll
+            for (int u = 0; u < L; ++u) {
+                const I c = __shfl_sync(FULL, col, u, L);
+                if (u < cnt && col_ok) {
                     const uint4 raw = ldg_nc_v4_hint(bcol + (int64_t)c * ldb, pol_b);
                     memcpy(&bv[u], &raw, 16);
                 }
             }
 #pragma unroll
-            for (int u = 0; u < U; ++u) {
-                const T v = __shfl_sync(FULL, val, (j + u) & 31);
-                if (j + u < take) {
+            for (int u = 0; u < L; ++u) {
+                const T v = __shfl_sync(FULL, val, u, L);
+                if (u < cnt) {
 #pragma unroll
                     for (int k = 0; k < VEC; ++k) acc.v[k] = add_rn(acc.v[k], mul_rn(v, bv[u].v[k]));
                 }
             }
         }
-        base += take;
-        if (take < 32 || base >= end) break;  // reached the panel boundary or the end of the row
-        const int64_t rem = end - base;
-        cnt = rem > 32 ? 32 : (int)rem;
-        col = 0;
-        if (lane < cnt) {
-            col = ldg_stream(a_indices + base + lane);
-            val = ldg_stream(a_data + base + lane);
+        // pass 0 writes every row (rows without entries get +0, as in K1); later passes only rows they touched
+        if (row_ok && col_ok && (first || s < e)) {
+            uint4 u;
+            memcpy(&u, &acc, 16);
+            stg_cs_v4(crow, u);
         }
-        m = __ballot_sync(FULL, lane < cnt && (int64_t)col < col_hi);
-        take = __popc(m);
-        if (take == 0) break;
-    }
-    if (!last && blockIdx.y == 0 && lane == 0) cursor_out[row] = (I)base;
-    if (col_ok) {
-        uint4 u;
-        memcpy(&u, &acc, 16);
-        stg_cs_v4(crow, u);
+        s = sn;
+        e = en;
+        sn = s2;
+        en = e2;
+        colv = colv_n;
+        valv = valv_n;
     }
 }
 
@@ -141,27 +217,115 @@ __global__ void max_row_kernel(int64_t M, const I *__restrict__ indptr, unsigned
     if ((threadIdx.x & 31) == 0 && m) atomicMax(out, m);
 }
 
-template <typename T, typename I>
-static int run_panels(int64_t M, int64_t K, int64_t N, const void *ad, const void *ai, const void *ap, const void *b,
-                      int64_t ldb, void *out, int64_t ldc, int n_panels, cudaStream_t s) {
+// ---------------------------------------------------------------------------
+// selection and host-side driver
+// ---------------------------------------------------------------------------
+// Defaults from tools/tune_panels.py on an H100 80GB HBM3 at 700 W (one-pass kernel 16.65 ms at C2 in the same run):
+// C2 with 128-byte tiles takes 13.50 / 12.28 / 11.86 / 12.90 / 14.14 ms at 12 / 16 / 24 / 32 / 48 MB per pass; 64-byte
+// tiles are never faster than 16.7 ms (the A stream is read once per tile) and 256-byte tiles not faster than 13.2 ms
+// (twice the panels for the same L2 footprint).  With every column inside one 16 MB panel (all gathers L2 hits) the
+// passes take 9.82 ms: the L2 line rate, not DRAM, is now the limit.  The passes carry a fixed cost (C read and
+// written 2P-1 times, offsets), so they lose at low reuse: 3.76 vs 1.87 ms at nnz / K = 10, 5.98 vs 5.22 ms at 30.
+// They did not gain for fp64 (N = 64: 17.89 vs 17.85 ms), so the automatic choice is fp32 only.
+constexpr int64_t kPanelBytes = 24ll << 20;  // B bytes (one panel x one tile) per pass
+constexpr int kTileBytes = 128;               // column tile: one cache line per gather
+constexpr int kL2Multiple = 2;                // tiled only when B is larger than this many L2s ...
+constexpr int64_t kMinReuse = 64;             // ... and each B row is used at least this often (nnz / K)
+
+static int64_t g_panel_bytes = 0;  // b2s_spmm_set_tiling (0 = default)
+static int g_tile_bytes = 0;
+int g_tile_hint = 1;  // 0: the passes load B with no L2 policy (b2s_spmm_set_variant(4, ...), for the sweep)
+
+static int64_t l2_bytes() {
+    static int64_t cached = 0;
+    if (cached == 0) {
+        int dev = 0, v = 0;
+        if (cudaGetDevice(&dev) == cudaSuccess && cudaDeviceGetAttribute(&v, cudaDevAttrL2CacheSize, dev) == cudaSuccess &&
+            v > 0)
+            cached = v;
+        else
+            cached = 50ll << 20;  // H100 SXM
+    }
+    return cached;
+}
+
+// lanes per row group for a tile of `tile_bytes` (clamped to what N needs)
+static int tile_lanes(int64_t N, size_t es) {
+    const int tb = g_tile_bytes > 0 ? g_tile_bytes : kTileBytes;
+    int lanes = tb <= 64 ? 4 : (tb <= 128 ? 8 : 16);
+    const int64_t packs = (N * (int64_t)es + 15) / 16;
+    while (lanes > 4 && packs <= lanes / 2) lanes /= 2;
+    return lanes;
+}
+
+// Number of K panels of the tiled path for this call, or 0 for the one-pass kernel.
+static int choose_panels(int dtype, int64_t K, int64_t N, int64_t nnz, bool vec_ok, int long_rows, int n_panels,
+                         int rows_sorted) {
+    if ((dtype != B2S_F32 && dtype != B2S_F64) || !vec_ok || rows_sorted == 0) return 0;
+    if (n_panels >= 2) return n_panels;
+    if (n_panels != 0 || long_rows || nnz < 0 || K <= 0 || dtype != B2S_F32) return 0;
+    const size_t es = dtype_size(dtype);
+    if (K * N * (int64_t)es <= kL2Multiple * l2_bytes() || nnz < kMinReuse * K) return 0;
+    const int64_t slice_row = (int64_t)tile_lanes(N, es) * 16;  // B bytes of one row within one tile
+    const int64_t budget = g_panel_bytes > 0 ? g_panel_bytes : kPanelBytes;
+    const int64_t P = (K * slice_row + budget - 1) / budget;
+    return (int)(P < 1 ? 1 : (P > 4096 ? 4096 : P));
+}
+
+template <typename T, typename I, int L>
+static int launch_passes(int64_t M, int64_t N, const void *ad, const void *ai, const I *off, int P, const void *b,
+                         int64_t ldb, void *out, int64_t ldc, const int *unsorted, cudaStream_t s) {
     constexpr int VEC = 16 / sizeof(T);
-    I *cursor = nullptr;
-    int rc = scratch_alloc((void **)&cursor, (size_t)M * sizeof(I) * 2, s);
+    constexpr int64_t TILE = (int64_t)L * VEC;  // columns per tile
+    auto kern = spmm_tile_pass_kernel<T, I, L>;
+    int occ = 1;
+    B2S_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, kern, 256, 0));
+    int64_t blocks = (int64_t)num_sms() * (occ < 1 ? 1 : occ);
+    const int64_t need = (M + 8 * (32 / L) - 1) / (8 * (32 / L));
+    if (blocks > need) blocks = need;
+    for (int64_t c0 = 0; c0 < N; c0 += TILE) {
+        for (int p = 0; p < P; ++p) {
+            kern<<<(unsigned)blocks, 256, 0, s>>>(M, N, (const T *)ad, (const I *)ai, off + (int64_t)p * M,
+                                                  off + (int64_t)(p + 1) * M, (const T *)b, ldb, (T *)out, ldc, c0,
+                                                  p == 0 ? 1 : 0, g_tile_hint, unsorted);
+            B2S_CHECK_LAUNCH();
+        }
+    }
+    return B2S_OK;
+}
+
+template <typename T, typename I>
+static int run_tiled(int dtype, int idx_bytes, int64_t M, int64_t K, int64_t N, const void *ad, const void *ai,
+                     const void *ap, const void *b, int64_t ldb, void *out, int64_t ldc, int P, cudaStream_t s) {
+    // scratch: the unsorted flag (16 bytes) then the (P+1) x M offsets
+    void *scr = nullptr;
+    int rc = scratch_alloc(&scr, 16 + (size_t)(P + 1) * M * sizeof(I), s);
     if (rc) return rc;
-    const int64_t gx = (M + 7) / 8;
-    const int64_t gy = (N + 32 * VEC - 1) / (32 * VEC);
-    B2S_REQUIRE(gx <= 2147483647LL && gy <= 65535, B2S_ERR_OVERFLOW, "spmm_panels: grid too large");
-    dim3 grid((unsigned)gx, (unsigned)gy);
-    const int64_t width = (K + n_panels - 1) / n_panels;
-    for (int p = 0; p < n_panels; ++p) {
-        const int64_t hi = (p + 1 == n_panels) ? (int64_t)1 << 62 : (int64_t)(p + 1) * width;
-        spmm_panel_kernel<T, I, 8><<<grid, 256, 0, s>>>(M, N, (const T *)ad, (const I *)ai, (const I *)ap,
-                                                       cursor + (size_t)((p + 1) & 1) * M, cursor + (size_t)(p & 1) * M,
-                                                       (const T *)b, ldb, (T *)out, ldc, hi, p == 0 ? 1 : 0,
-                                                       p + 1 == n_panels ? 1 : 0);
+    int *flag = (int *)scr;
+    I *off = (I *)((char *)scr + 16);
+    B2S_CUDA(cudaMemsetAsync(flag, 0, 4, s));
+    {
+        int64_t blocks = (M * 32 + 255) / 256;
+        const int64_t cap = (int64_t)num_sms() * 16;
+        if (blocks > cap) blocks = cap;
+        const int64_t width = (K + P - 1) / P;
+        panel_offsets_kernel<I><<<(unsigned)blocks, 256, 0, s>>>(M, (const I *)ap, (const I *)ai, width < 1 ? 1 : width,
+                                                                P, off, flag);
         B2S_CHECK_LAUNCH();
     }
-    return scratch_free(cursor, s);
+    const int lanes = tile_lanes(N, sizeof(T));
+    if (lanes == 4) rc = launch_passes<T, I, 4>(M, N, ad, ai, off, P, b, ldb, out, ldc, flag, s);
+    else if (lanes == 8) rc = launch_passes<T, I, 8>(M, N, ad, ai, off, P, b, ldb, out, ldc, flag, s);
+    else rc = launch_passes<T, I, 16>(M, N, ad, ai, off, P, b, ldb, out, ldc, flag, s);
+    if (rc) return rc;
+    // the one-pass kernel, which returns at entry unless some row was unsorted
+    set_call_skew(0);
+    set_call_guard(flag);
+    rc = spmm_csr_dense_impl(dtype, idx_bytes, M, K, N, ad, ai, ap, b, ldb, out, ldc, s);
+    set_call_guard(nullptr);
+    set_call_skew(-1);
+    if (rc) return rc;
+    return scratch_free(scr, s);
 }
 
 }  // namespace b2s
@@ -170,7 +334,7 @@ using namespace b2s;
 
 extern "C" {
 
-/* 1 if every row of the CSR has non-decreasing column indices (precondition of the panel passes). Synchronises. */
+/* 1 if every row of the CSR has non-decreasing column indices. Synchronises. */
 int b2s_csr_rows_sorted(int idx_bytes, int64_t M, const void *indptr_dev, const void *indices_dev, int *sorted_host,
                         void *stream) {
     B2S_REQUIRE(sorted_host != nullptr, B2S_ERR_INVALID, "csr_rows_sorted: NULL output");
@@ -219,11 +383,20 @@ int b2s_csr_max_row_nnz(int idx_bytes, int64_t M, const void *indptr_dev, int64_
     return B2S_OK;
 }
 
+int b2s_spmm_set_tiling(int64_t panel_bytes, int tile_bytes) {
+    B2S_REQUIRE(panel_bytes >= 0 && (tile_bytes == 0 || tile_bytes == 64 || tile_bytes == 128 || tile_bytes == 256),
+                B2S_ERR_INVALID, "spmm_set_tiling: panel_bytes >= 0, tile_bytes in {0, 64, 128, 256}");
+    g_panel_bytes = panel_bytes;
+    g_tile_bytes = tile_bytes;
+    return B2S_OK;
+}
+
 /*
- * K1 with explicit scheduling control.  n_panels <= 1: the one-pass kernel (same as b2s_spmm_csr_dense).
- * n_panels >= 2: column-panel passes (rows MUST be sorted by column -- check with b2s_csr_rows_sorted; 16-byte aligned
- * fp32/fp64 operands with N * sizeof(T) a multiple of 16); n_panels == 0: choose automatically from the size of B
- * (about 48 MB of B per panel) when `rows_sorted` is 1 and the matrix has enough entries per row (`nnz` >= 0 known).
+ * K1 with explicit scheduling control.  n_panels == 1: the one-pass kernel.  n_panels >= 2: tiled passes with that many
+ * K panels (fp32/fp64 with 16-byte aligned operands; otherwise the one-pass kernel).  n_panels == 0: tiled passes for
+ * fp32 when B is larger than kL2Multiple L2s and nnz >= kMinReuse x K (P from the panel budget), else the one-pass
+ * kernel.
+ * rows_sorted is advisory (0 = known unsorted: skip the passes); the passes check the order on the device themselves.
  */
 int b2s_spmm_csr_dense_ex(int dtype, int idx_bytes, int64_t M, int64_t K, int64_t N, int64_t nnz,
                           const void *a_data_dev, const void *a_indices_dev, const void *a_indptr_dev,
@@ -233,29 +406,22 @@ int b2s_spmm_csr_dense_ex(int dtype, int idx_bytes, int64_t M, int64_t K, int64_
     const size_t es = dtype_size(dtype);
     const bool vec_ok = (dtype == B2S_F32 || dtype == B2S_F64) && es != 0 && (N * es) % 16 == 0 &&
                         (ldb * es) % 16 == 0 && (ldc * es) % 16 == 0 && (((uintptr_t)b_dev | (uintptr_t)out_dev) & 15) == 0;
-    if (n_panels == 0) {
-        // Measured at C2 on an H100 SXM (700 W): 16.19 ms one-pass vs 16.51 / 15.71 / 17.27 / 24.74 ms with
-        // 2 / 8 / 16 / 32 panels.  The one-pass kernel already moves 0.97 of the data-sheet HBM bandwidth in gather-model
-        // bytes, so turning DRAM misses into L2 hits buys at most 3 % (8 panels), and every extra pass adds its C
-        // read-modify-write.  The automatic choice stays the one-pass kernel; panels are available on explicit request.
-        (void)nnz;
-        n_panels = 1;
-    }
-    if (n_panels <= 1 || !vec_ok || M == 0 || N == 0) {
+    B2S_REQUIRE(M >= 0 && K >= 0 && N >= 0, B2S_ERR_INVALID, "spmm: negative dimension");
+    B2S_REQUIRE(ldb >= N && ldc >= N, B2S_ERR_INVALID, "spmm: ldb/ldc smaller than N");
+    const int P = (M == 0 || N == 0) ? 0 : choose_panels(dtype, K, N, nnz, vec_ok, long_rows, n_panels, rows_sorted);
+    if (P == 0) {
         set_call_skew(long_rows ? 1 : 0);
         const int rc = spmm_csr_dense_impl(dtype, idx_bytes, M, K, N, a_data_dev, a_indices_dev, a_indptr_dev, b_dev,
                                            ldb, out_dev, ldc, s);
         set_call_skew(-1);
         return rc;
     }
-    B2S_REQUIRE(rows_sorted == 1, B2S_ERR_INVALID, "spmm panels: rows must be sorted by column (rows_sorted=1)");
-    B2S_REQUIRE(idx_bytes == 4 || idx_bytes == 8, B2S_ERR_INVALID, "spmm panels: idx_bytes");
-    if (dtype == B2S_F32) {
-        return idx_bytes == 4 ? run_panels<float, int32_t>(M, K, N, a_data_dev, a_indices_dev, a_indptr_dev, b_dev, ldb, out_dev, ldc, n_panels, s)
-                              : run_panels<float, int64_t>(M, K, N, a_data_dev, a_indices_dev, a_indptr_dev, b_dev, ldb, out_dev, ldc, n_panels, s);
-    }
-    return idx_bytes == 4 ? run_panels<double, int32_t>(M, K, N, a_data_dev, a_indices_dev, a_indptr_dev, b_dev, ldb, out_dev, ldc, n_panels, s)
-                          : run_panels<double, int64_t>(M, K, N, a_data_dev, a_indices_dev, a_indptr_dev, b_dev, ldb, out_dev, ldc, n_panels, s);
+    B2S_REQUIRE(idx_bytes == 4 || idx_bytes == 8, B2S_ERR_INVALID, "spmm: idx_bytes must be 4 or 8");
+#define B2S_TILED(T, I) \
+    run_tiled<T, I>(dtype, idx_bytes, M, K, N, a_data_dev, a_indices_dev, a_indptr_dev, b_dev, ldb, out_dev, ldc, P, s)
+    if (dtype == B2S_F32) return idx_bytes == 4 ? B2S_TILED(float, int32_t) : B2S_TILED(float, int64_t);
+    return idx_bytes == 4 ? B2S_TILED(double, int32_t) : B2S_TILED(double, int64_t);
+#undef B2S_TILED
 }
 
 }  // extern "C"
