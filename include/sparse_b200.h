@@ -321,6 +321,41 @@ int b2s_mttkrp_mode(int dtype, int idx_bytes, int order, int mode, int64_t nnz, 
                     const void *const *coords_host, const void *vals_dev, const void *const *factors_host,
                     const int64_t *ld_host, void *out_dev, int64_t ldo, void *stream);
 
+/* ---- masked sparse x sparse product (K11, masked_spgemm.cu; examples/triangles_example.py) ------------------------
+ * out_vals[p] = value of mask * (A @ B) at every stored mask entry p, given the mask as CSR (m_indptr over the M rows,
+ * m_cols, m_vals already in the output dtype `dtype_out`), A as CSR (M x K) and B^T as CSR (N x K, i.e. B by
+ * columns), both in the product dtype `dtype_c`.  Writes exactly nnz_m values, in the mask's stored order; dropping
+ * the results that are bitwise +0 is left to the caller (the prune compaction).  The rows of A and B^T must hold
+ * strictly increasing indices (b2s_masked_spgemm_sorted checks it).  No stream synchronisation.
+ * Supported (dtype_c, dtype_out): (f32, f32), (f32, f64), (f64, f64), (i32, i32), (i32, i64), (i32, f64), (i64, i64),
+ * (i64, f64) -- every pair result_type(a, b) / result_type(mask, result_type(a, b)) can produce within f32, f64, i32,
+ * i64.
+ *
+ * Fixed order of operations, for each stored mask entry (i, j, m) (results are reproducible bit for bit, whatever the
+ * grid, the staging capacity or the stream):
+ *  1. c' = ((+0 + a_ik1 * b_k1j) + a_ik2 * b_k2j) + ... in dtype_c, over the k present in both row i of A and column j
+ *     of B, in ascending k; every product and every sum rounded separately, no FMA contraction; integers wrap.  An
+ *     empty intersection gives c' = +0.
+ *  2. v = T(m) * T(c'), rounded in T = dtype_out.
+ *  3. out_vals[p] = v.  The entry is kept iff bits(v) != bits(+0) (for integers: v != 0).
+ * This is the order of the unfused path: the Gustavson product (K4) adds sums[j] += a_ik * b_kj from +0 in A's row
+ * order (ascending k for canonical A), prunes sums that are bitwise +0 (which the multiply then sees as the fill
+ * value +0, the same c'), and the elementwise multiply computes T(m) * T(c) and drops bitwise +0 results. */
+int b2s_masked_spgemm(int dtype_c, int dtype_out, int idx_bytes, int64_t M, int64_t N, int64_t K, int64_t nnz_m,
+                      const void *m_indptr_dev, const void *m_cols_dev, const void *m_vals_dev,
+                      const void *a_indptr_dev, const void *a_cols_dev, const void *a_vals_dev, int64_t nnz_bt,
+                      const void *bt_indptr_dev, const void *bt_cols_dev, const void *bt_vals_dev, void *out_vals_dev,
+                      void *stream);
+/* test hook: A entries staged per segment (1 .. 512; 0 = default 512).  Small values force the segment path. */
+int b2s_masked_spgemm_set_stage(int cap);
+/* *sorted_host = 1 iff every row of A (M rows) and of B^T (N rows) holds strictly increasing indices; a NULL indptr
+ * skips that operand.  One stream synchronisation. */
+int b2s_masked_spgemm_sorted(int idx_bytes, int64_t M, const void *a_indptr_dev, const void *a_cols_dev, int64_t N,
+                             const void *bt_indptr_dev, const void *bt_cols_dev, int *sorted_host, void *stream);
+/* flags[q] = 1 iff query[q] occurs in the ascending array set[0..ns) (restriction of a result to a mask's pattern). */
+int b2s_keys_member(const int64_t *query_dev, int64_t nq, const int64_t *set_dev, int64_t ns, uint8_t *flags_dev,
+                    void *stream);
+
 /* ---- copy-engine exchange of a row-sharded dense operand (peer.cu; SURVEY.md s8(e), no reference counterpart: the
  * reference is single-process) ------------------------------------------------------------------------------------
  * b2s_peer_alloc: cudaMalloc'ed (IPC-exportable) device buffer; b2s_peer_export writes its 64-byte CUDA IPC handle;

@@ -9,6 +9,10 @@ BLAS / reduceat order, so parity is tolerance-based (rtol 1e-5 f32, 1e-12 f64 in
 
 mttkrp_mode(X, factors, mode) generalises mttkrp to any mode of a tensor of order 2..8 (the CP-ALS step); it has no
 counterpart in the reference beyond the unfused broadcast expression / einsum.
+
+masked_matmul(mask, a, b) == mask * (a @ b) at mask's stored positions, for sparse a and b: the masked SpGEMM of
+examples/triangles_example.py (sum(a @ a * a) / 6) and of the GraphBLAS masked mxm.  It never forms the product
+a @ b, so its memory is O(nnz(mask)), and it is bit-identical to the unfused expression on the mask's pattern.
 """
 from __future__ import annotations
 
@@ -20,7 +24,7 @@ from numpy.exceptions import AxisError
 from . import _device as D
 from . import _kernels as Kn
 from ._coo import COO
-from ._dot import _coo_as_csr, _dense_dev, _narrow_idx, _return_dense
+from ._dot import _coo_as_csr, _csr_arrays, _dense_dev, _narrow_idx, _return_dense
 from ._sparse_array import SparseArray
 from ._utils import check_zero_fill_value
 
@@ -181,3 +185,117 @@ def mttkrp_mode(X, factors, mode):
         fac = [None if m == mode else _dense_dev(factors[m], T) for m in range(N)]
         out = Kn.mttkrp_mode(coords, Kn.cast(vals, T), fac, mode, rows, R)
     return _return_dense(out, [f for f in factors if f is not None])
+
+
+# Test hook: True keeps masked_matmul's index arrays int64 even when every extent and nnz fit int32.
+_FORCE_WIDE_INDEX_MASKED = False
+
+_MASKED_DTYPES = tuple(np.dtype(d) for d in ("float32", "float64", "int32", "int64"))
+
+
+def _rows_of_b(b, Tc):
+    """(B^T as CSR arrays (vals, indices, indptr), whether they are b's own stored arrays)."""
+    from ._gcxs import GCXS
+
+    if isinstance(b, GCXS):
+        if b.compressed_axes == (1,):
+            return _csr_arrays(b._2d_transpose(), Tc), True  # O(1): CSC of b is the CSR of b^T
+        return _csr_arrays(b.change_compressed_axes((1,))._2d_transpose(), Tc), False  # one conversion per call
+    return _coo_as_csr(b, Tc, by_col=True), False
+
+
+def _rows_of_a(a, Tc):
+    """(A as CSR arrays (vals, indices, indptr), whether they are a's own stored arrays)."""
+    from ._gcxs import GCXS
+
+    if isinstance(a, GCXS):
+        if a.compressed_axes == (0,):
+            return _csr_arrays(a, Tc), True
+        return _csr_arrays(a.change_compressed_axes((0,)), Tc), False
+    return _coo_as_csr(a, Tc), False
+
+
+def _masked_unfused(mask, a, b, T):
+    """mask * (a @ b) through the package's own product and multiply, restricted to mask's stored positions."""
+    from ._gcxs import GCXS
+
+    r = mask * (a @ b)
+    r = r.tocoo() if isinstance(r, GCXS) else r
+    mc = mask.tocoo() if isinstance(mask, GCXS) else mask
+    _, data = r._dev()
+    keys = r.sorted_keys()
+    flags = Kn.keys_member(keys, mc.sorted_keys())
+    pos, total = Kn.scan_flags(flags)
+    res = COO._from_device(None, Kn.cast(Kn.compact(data, flags, pos, total), T),
+                           mask.shape, T.type(0), keys=Kn.compact(keys, flags, pos, total))
+    return res.asformat("gcxs", compressed_axes=mask.compressed_axes) if isinstance(mask, GCXS) else res
+
+
+def masked_matmul(mask, a, b):
+    """Masked sparse x sparse product: the value of ``mask * (a @ b)`` at every stored position of `mask`, without
+    forming ``a @ b`` (examples/triangles_example.py: ``masked_matmul(A, A, A).sum() / 6`` counts the triangles of a
+    symmetric adjacency matrix A).
+
+    `mask` (M, N), `a` (M, K) and `b` (K, N) are 2-D COO or GCXS arrays with a zero fill value.  The result has
+    `mask`'s format (a GCXS result keeps ``mask.compressed_axes``) and dtype result_type(mask.dtype, result_type(a.dtype,
+    b.dtype)); both dtypes must be float32, float64, int32 or int64.  Values are bit-identical to the unfused
+    expression at the mask's positions: c = sum over k of a[i, k] * b[k, j] in ascending k from +0 (each product and sum
+    rounded, integers wrap), then mask[i, j] * c, and entries whose result is bitwise +0 are not stored
+    (include/sparse_b200.h, b2s_masked_spgemm).  The memory is O(nnz(mask) + nnz(a) + nnz(b)).
+
+    One difference from ``mask * (a @ b)``: the unfused expression also stores entries OUTSIDE mask's pattern, ``0 * c =
+    -0.0`` where (a @ b)[i, j] is negative and NaN where it is inf or NaN, because pruning compares bit patterns (-0.0
+    is not +0).  masked_matmul has GraphBLAS masked semantics and never produces those entries; where ``a @ b`` is
+    non-negative and finite outside the mask (graphs, for instance) the two results are equal in full.
+
+    Layout costs: the kernel reads a by rows and b by columns.  A CSR / COO `a` and a CSC / COO `b` are used as they are
+    (a COO `b` is sorted by column once per call); a CSC `a` or a CSR `b` is converted once per call, at the cost of a
+    format conversion of that operand.  For a symmetric adjacency matrix, pass ``A.T`` (an O(1) view) as `b`.
+    GCXS operands whose rows hold unsorted or repeated indices (possible when the arrays are built by hand) are summed
+    in a different order by the unfused path; such calls are detected with one device check and computed as the
+    unfused expression restricted to the mask's pattern.
+    """
+    from ._gcxs import GCXS
+
+    for name, x in (("mask", mask), ("a", a), ("b", b)):
+        if not isinstance(x, (COO, GCXS)) or x.ndim != 2:
+            raise TypeError(f"masked_matmul: `{name}` must be a 2-D sparse_b200 COO or GCXS array")
+    check_zero_fill_value(mask, a, b)
+    M, N = mask.shape
+    if a.shape[0] != M or b.shape[1] != N or a.shape[1] != b.shape[0]:
+        raise ValueError(f"masked_matmul: shape mismatch mask{mask.shape}, a{a.shape}, b{b.shape}")
+    K = a.shape[1]
+    Tc = np.result_type(a.dtype, b.dtype)
+    T = np.result_type(mask.dtype, Tc)
+    if Tc not in _MASKED_DTYPES or T not in _MASKED_DTYPES:
+        raise TypeError(f"masked_matmul: dtypes ({mask.dtype}, {a.dtype}, {b.dtype}) are outside the CUDA dtype "
+                        "matrix (float32, float64, int32, int64)")
+    was_gcxs = isinstance(mask, GCXS)
+    if mask.nnz == 0:
+        res = COO._from_device(None, Kn.full(0, 0, T), mask.shape, T.type(0), keys=Kn.full(0, 0, np.int64))
+        return res.asformat("gcxs", compressed_axes=mask.compressed_axes) if was_gcxs else res
+    (av, ai, ap), a_own = _rows_of_a(a, Tc)
+    (bv, bi, bp), b_own = _rows_of_b(b, Tc)
+    if was_gcxs:
+        mv, mi_own, mp_own = mask._dev()
+        mvals, mi, mp = Kn.cast(mv, T), mi_own, mp_own
+    else:
+        mvals, mi, mp = _coo_as_csr(mask, T)
+    limit = 2**63 if _FORCE_WIDE_INDEX_MASKED else max(M, N, K, mask.nnz, a.nnz, b.nnz)
+    mi, mp, ai, ap, bi, bp = _narrow_idx(mi, mp, ai, ap, bi, bp, limit=limit)
+    if (a_own or b_own) and not Kn.masked_spgemm_sorted(ap if a_own else None, ai if a_own else None, M,
+                                                        bp if b_own else None, bi if b_own else None, N):
+        return _masked_unfused(mask, a, b, T)
+    if was_gcxs:
+        # a CSC mask is the CSR of mask^T: (mask o (a @ b))^T = mask^T o (b^T @ a^T), still summed in ascending k
+        if mask.compressed_axes == (0,):
+            out = Kn.masked_spgemm(mp, mi, mvals, ap, ai, av, bp, bi, bv, M, N, K)
+        else:
+            out = Kn.masked_spgemm(mp, mi, mvals, bp, bi, bv, ap, ai, av, N, M, K)
+        res = GCXS._from_device(out, mi_own, mp_own, mask.shape, mask.compressed_axes, T.type(0))
+        res._prune()  # mask * (a @ b) drops results that are bitwise +0 (the prune compaction)
+        return res
+    out = Kn.masked_spgemm(mp, mi, mvals, ap, ai, av, bp, bi, bv, M, N, K)
+    res = COO._from_device(mask._coords, out, mask.shape, T.type(0), keys=mask.sorted_keys())
+    res._canonicalise(check_sort=False, sum_dups=False, prune=True)  # drops bitwise +0 results, as the multiply does
+    return res

@@ -684,3 +684,50 @@ def mttkrp_mode(coords, vals, factors, mode, rows, R):
                                      vp(D.ptr(out)), i64(R), _sp())
     _lib.check(rc, "b2s_mttkrp_mode")
     return out
+
+
+# ------------------------------------------------------------------------------------------------
+# K11 masked SpGEMM
+# ------------------------------------------------------------------------------------------------
+def masked_spgemm(m_indptr, m_cols, m_vals, a_indptr, a_cols, a_vals, bt_indptr, bt_cols, bt_vals, M, N, K):
+    """out_vals[p] = value of mask * (A @ B) at stored mask entry p, in the fixed order of b2s_masked_spgemm
+    (examples/triangles_example.py).  The mask is CSR with values in the output dtype; A (M x K) and B^T (N x K) are
+    CSR in the product dtype with strictly increasing indices per row; all index arrays share one width."""
+    t = _t()
+    dc, do = D.np_dtype(a_vals), D.np_dtype(m_vals)
+    assert bt_vals.dtype == a_vals.dtype
+    assert all(x.dtype == m_cols.dtype for x in (m_indptr, a_indptr, a_cols, bt_indptr, bt_cols))
+    out = t.empty_like(m_vals)
+    rc = _lib.load().b2s_masked_spgemm(
+        i32(D.dtype_code(dc)), i32(D.dtype_code(do)), i32(_idx_bytes(m_cols)), i64(M), i64(N), i64(K),
+        i64(m_vals.shape[0]), vp(D.ptr(m_indptr)), vp(D.ptr(m_cols)), vp(D.ptr(m_vals)), vp(D.ptr(a_indptr)),
+        vp(D.ptr(a_cols)), vp(D.ptr(a_vals)), i64(bt_vals.shape[0]), vp(D.ptr(bt_indptr)), vp(D.ptr(bt_cols)),
+        vp(D.ptr(bt_vals)), vp(D.ptr(out)), _sp())
+    _lib.check(rc, "b2s_masked_spgemm")
+    return out
+
+
+def masked_spgemm_set_stage(cap: int = 0):
+    """Test hook: A entries staged per segment of masked_spgemm (0 = default); small values force the segment path."""
+    _lib.check(_lib.load().b2s_masked_spgemm_set_stage(i32(cap)))
+
+
+def masked_spgemm_sorted(a_indptr, a_cols, M, bt_indptr, bt_cols, N) -> bool:
+    """True when every row of A and of B^T holds strictly increasing indices (None skips an operand); one sync."""
+    r = ctypes.c_int(1)
+    idx = a_cols if a_cols is not None else bt_cols
+    _lib.check(_lib.load().b2s_masked_spgemm_sorted(
+        i32(_idx_bytes(idx)), i64(M), vp(D.ptr(a_indptr) if a_indptr is not None else 0),
+        vp(D.ptr(a_cols) if a_cols is not None else 0), i64(N),
+        vp(D.ptr(bt_indptr) if bt_indptr is not None else 0), vp(D.ptr(bt_cols) if bt_cols is not None else 0),
+        ctypes.byref(r), _sp()), "b2s_masked_spgemm_sorted")
+    return bool(r.value)
+
+
+def keys_member(query, keys):
+    """uint8 flags: query[q] occurs in the ascending int64 array `keys`."""
+    t = _t()
+    flags = t.empty(query.shape[0], dtype=t.uint8, device=query.device)
+    _lib.check(_lib.load().b2s_keys_member(vp(D.ptr(query)), i64(query.shape[0]), vp(D.ptr(keys)), i64(keys.shape[0]),
+                                           vp(D.ptr(flags)), _sp()), "b2s_keys_member")
+    return flags

@@ -5,7 +5,9 @@ Device-resident inputs (generated with seeded torch generators on the GPU), wall
 torch.cuda.synchronize() because the public calls contain their own size-returning syncs.
 Prints one line per config as it runs and the whole result as one JSON line at the end.
 
-    python tools/bench_configs.py [c1 c3 c3big red c4 c5 mttkrp mttkrp_mode]
+    python tools/bench_configs.py [c1 c3 c3big red c4 c5 mttkrp mttkrp_mode masked]
+
+`masked` (the masked SpGEMM, examples/triangles_example.py) runs only when named.
 """
 import json
 import os
@@ -274,8 +276,125 @@ def run(which=None, compact=False, parity=True):
             del contrib, wantm
         del Bt, Dm, Cm
         res.update(_mttkrp_mode_order3(rec, parity))
+    if "masked" in which:
+        res.update(_masked(rec, parity))
     torch.cuda.empty_cache()
     return res
+
+
+def _card():
+    """Name and power limit of the GPU, read next to the timings."""
+    import subprocess
+
+    q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader",
+                        "-i", str(DEV.index or 0)], capture_output=True, text=True)
+    return q.stdout.strip() or torch.cuda.get_device_name(DEV)
+
+
+def _graph_from_edges(n, i, j):
+    """Symmetric 0/1 float32 adjacency matrix (COO) of the edges (i, j), without self-loops or duplicates."""
+    keep = i != j
+    i, j = i[keep], j[keep]
+    keys = torch.unique(torch.cat([i * n + j, j * n + i]))
+    coords = torch.stack([torch.div(keys, n, rounding_mode="floor"), keys % n])
+    return sp.COO(coords, torch.ones(keys.numel(), device=DEV, dtype=torch.float32), shape=(n, n),
+                  has_duplicates=False, sorted=True)
+
+
+def _rmat_edges(n_log2, m, seed, probs=(0.57, 0.19, 0.19, 0.05)):
+    g = torch.Generator(device=DEV).manual_seed(seed)
+    i = torch.zeros(m, dtype=torch.int64, device=DEV)
+    j = torch.zeros(m, dtype=torch.int64, device=DEV)
+    cut = torch.tensor(np.cumsum(probs)[:3], device=DEV, dtype=torch.float32)
+    for _ in range(n_log2):
+        q = torch.bucketize(torch.rand(m, generator=g, device=DEV), cut)
+        i = i * 2 + (q >= 2).to(torch.int64)
+        j = j * 2 + (q % 2).to(torch.int64)
+    return i, j
+
+
+def _masked(rec, parity):
+    """Masked SpGEMM on graphs (mask = a = b = the adjacency matrix A, f32): masked_matmul(A, A, A) against the
+    unfused A * (A @ A).  Byte model per call (from the degrees d_i of A, with nnz = sum d_i):
+      mask stream    nnz * (4 index + 4 value + 4 result) + indptr
+      A staging      nnz * (4 + 4): every row of A is staged once per chunk that touches its mask row
+      B^T indices    sum over mask entries (i, j) of d_j * 4 = sum_j d_j^2 * 4 (plus 8 B of extent per entry)
+      value gathers  4 B per match; a match of entry (i, j) is a triangle through the edge, 6 per triangle
+    Unfused memory: K4's upper-bound layout holds min(P_i, n) (index + value) slots per row (P_i = sum of the
+    degrees of the row's neighbours) and its result (int64 index + value) per product, then the multiply merges the
+    whole product with the mask.  The unfused call is run in row blocks to keep the footprint moderate: rows of
+    A * (A @ A) depend only on the same rows of the mask and of A, so the values are those of one call."""
+    sys.path.insert(0, os.path.join(ROOT, "tests"))
+    import _mock_masked as MM
+
+    out = {}
+    card = _card()
+    n_log2 = 20
+    n = 1 << n_log2
+    m = n * 16
+    g = torch.Generator(device=DEV).manual_seed(51)
+    uniform = _graph_from_edges(n, torch.randint(0, n, (m,), generator=g, device=DEV),
+                                torch.randint(0, n, (m,), generator=g, device=DEV))
+    rmat = _graph_from_edges(n, *_rmat_edges(n_log2, m, 52))
+    for gname, A in (("uniform", uniform), ("R-MAT", rmat)):
+        A._dev()
+        keys = A.sorted_keys()
+        deg = torch.bincount(torch.div(keys, n, rounding_mode="floor"), minlength=n).to(torch.float64)
+        nnz = A.nnz
+        products = float((deg * deg).sum())  # sum_k |A_:,k| |A_k,:| for symmetric A
+        res = sp.masked_matmul(A, A, A)
+        matches = float(res._data_dev().double().sum())
+        alg = nnz * 12 + (n + 1) * 4 + nnz * 8 + products * 4 + nnz * 8 + matches * 4
+        p_row = torch.zeros(n, dtype=torch.float64, device=DEV).index_add_(
+            0, torch.div(keys, n, rounding_mode="floor"), deg[keys % n])
+        unfused_bytes = float(torch.clamp(p_row, max=n).sum()) * 8 + products * 12 + nnz * 16
+        name = f"masked_matmul {gname} graph 2^20 vertices, avg degree {nnz / n:.1f}, f32"
+        r = rec(name, lambda: sp.masked_matmul(A, A, A), nnz, "G_mask_entries_s", alg, reps=5)
+        r.update({"card": card, "mask_nnz": int(nnz), "products_unfused": int(products), "byte_model": int(alg),
+                  "unfused_memory_model_bytes": int(unfused_bytes), "triangles_fused": matches / 6,
+                  "max_degree": int(deg.max())})
+        if gname == "uniform":
+            blocks = 4
+            step = n // blocks
+            parts = [A[r0:r0 + step] for r0 in range(0, n, step)]
+            for p in parts:
+                p._dev()
+
+            def unfused():
+                return [p * (p @ A) for p in parts]
+
+            best, med = timeit(unfused, reps=3, warm=1)
+            ref = unfused()
+            rk = torch.cat([x.sorted_keys() + b * step * n for b, x in enumerate(ref)])
+            rv = torch.cat([x._data_dev() for x in ref])
+            inm = torch.isin(rk, keys)
+            fk, fv = res.sorted_keys(), res._data_dev()
+            r["unfused"] = {"ms_best": round(best, 4), "ms_median": round(med, 4), "row_blocks": blocks,
+                            "card": _card(), "triangles": float(rv.double().sum()) / 6,
+                            "entries_outside_mask": int((~inm).sum())}
+            r["parity"] = {"vs": "unfused A * (A @ A) of the package, restricted to the mask",
+                           "fused_equals_unfused_on_mask_bitwise": bool(
+                               torch.equal(rk[inm], fk) and torch.equal(rv[inm].view(torch.int32),
+                                                                           fv.view(torch.int32))),
+                           "triangles_equal": r["unfused"]["triangles"] == matches / 6}
+            r["speedup_vs_unfused"] = round(med / r["ms_median"], 2)
+            del ref, rk, rv, inm, parts
+        elif parity:
+            # six random rows and one long row (the degree nearest 512; the hubs take minutes in the CPU restatement)
+            rows = np.random.default_rng(53).choice(n, 6, replace=False).tolist() + [int((deg - 512).abs().argmin())]
+            mv, mi, mp = (x.cpu().numpy() for x in A.asformat("gcxs", compressed_axes=(0,))._dev())
+            full = torch.zeros(nnz, dtype=torch.float32, device=DEV)
+            full[torch.searchsorted(keys, res.sorted_keys())] = res._data_dev()
+            fullh = full.cpu().numpy()
+            ok = True
+            for i in rows:
+                pos, want = MM.order_contract(mp, mi, mv, mp, mi, mv, mp, mi, mv, rows=[i])
+                ok &= bool(np.array_equal(fullh[pos].view(np.uint32), want.view(np.uint32)))
+            r["parity"] = {"vs": "CPU restatement of the order (tests/_mock_masked.py) on 7 sampled rows",
+                           "sampled_rows_bit_exact": ok}
+        out[name] = r
+        del res, keys, deg, p_row
+    return out
 
 
 def _mttkrp_mode_order3(rec, parity):
