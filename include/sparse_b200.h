@@ -321,6 +321,30 @@ int b2s_mttkrp_mode(int dtype, int idx_bytes, int order, int mode, int64_t nnz, 
                     const void *const *coords_host, const void *vals_dev, const void *const *factors_host,
                     const int64_t *ld_host, void *out_dev, int64_t ldo, void *stream);
 
+/* ---- mode-n TTMc of a sparse tensor of order 2..8 (K12, mttkrp.cu; the Tucker / HOOI step, no reference
+ * counterpart) --------------------------------------------------------------------------------------------------------
+ * out[i, col] = sum over stored entries e with i_mode(e) = i of v_e * U_a[i_a(e), r_a] * U_b[i_b(e), r_b] * ..., where
+ * a < b < ... < z are the modes other than `mode`, U_m has ranks_host[m] columns, and the W = R_a * R_b * ... * R_z
+ * columns are in C order: col = ((r_a * R_b + r_b) * R_c + r_c) ... .  out is dense (rows x W, row stride ldo), fully
+ * written; ranks_host[mode] is not read.  Arguments otherwise as b2s_mttkrp_mode.  W <= B2S_TTMC_MAX_W: the combine
+ * kernel puts 32 columns on each of at most 65535 grid rows.  No stream synchronisation.
+ *
+ * Fixed order of operations (results are reproducible bit for bit, whatever the grid, SM count or stream):
+ *  1. The input is the same mode stream S_mode, cut into the same chunks of B2S_MTTKRP_CHUNK entries, as
+ *     b2s_mttkrp_mode's steps 1 and 3.
+ *  2. p_e[col] = ((...((v_e * U_a[i_a, r_a]) * U_b[i_b, r_b]) * ...) * U_z[i_z, r_z]) in ascending mode order, each
+ *     product rounded separately; no FMA contraction.  (The left-to-right association makes the prefix v_e * U_a * ...
+ *     * U_y common to the R_z columns that share r_a .. r_y; computing it once is bit-identical.)
+ *  3. Partials per (chunk, row) and row results over the chunks are b2s_mttkrp_mode's steps 4 and 5.
+ * With every R_m = R, column (r, r, ..., r) equals b2s_mttkrp_mode's column r bit for bit, and for order 2 the two
+ * results are equal.
+ */
+#define B2S_TTMC_MAX_W (65535 * 32)
+int b2s_ttmc_mode_max_width(void); /* returns B2S_TTMC_MAX_W */
+int b2s_ttmc_mode(int dtype, int idx_bytes, int order, int mode, int64_t nnz, int64_t rows, const int64_t *ranks_host,
+                  const void *const *coords_host, const void *vals_dev, const void *const *factors_host,
+                  const int64_t *ld_host, void *out_dev, int64_t ldo, void *stream);
+
 /* ---- masked sparse x sparse product (K11, masked_spgemm.cu; examples/triangles_example.py) ------------------------
  * out_vals[p] = value of mask * (A @ B) at every stored mask entry p, given the mask as CSR (m_indptr over the M rows,
  * m_cols, m_vals already in the output dtype `dtype_out`), A as CSR (M x K) and B^T as CSR (N x K, i.e. B by

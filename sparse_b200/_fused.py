@@ -8,7 +8,8 @@ intermediate and the nnz x J broadcast products.  Floating-point association dif
 BLAS / reduceat order, so parity is tolerance-based (rtol 1e-5 f32, 1e-12 f64 in the tests).
 
 mttkrp_mode(X, factors, mode) generalises mttkrp to any mode of a tensor of order 2..8 (the CP-ALS step); it has no
-counterpart in the reference beyond the unfused broadcast expression / einsum.
+counterpart in the reference beyond the unfused broadcast expression / einsum.  ttmc_mode(X, factors, mode) is its
+Kronecker counterpart, the TTMc step of Tucker / HOOI, with the same inputs and a rank per mode.
 
 masked_matmul(mask, a, b) == mask * (a @ b) at mask's stored positions, for sparse a and b: the masked SpGEMM of
 examples/triangles_example.py (sum(a @ a * a) / 6) and of the GraphBLAS masked mxm.  It never forms the product
@@ -130,6 +131,31 @@ def _mode_stream(X, mode):
     return stream
 
 
+def _tensor_and_factors(name, X, factors, mode):
+    """Checks shared by mttkrp_mode and ttmc_mode: (order N, mode in 0..N-1, the factors as a list with the other
+    modes' ones as NumPy arrays or device tensors, the other modes ascending)."""
+    from ._gcxs import GCXS
+
+    if not isinstance(X, (COO, GCXS)):
+        raise TypeError(f"{name}: `X` must be a sparse_b200 COO or GCXS array")
+    N = X.ndim
+    if not 2 <= N <= 8:
+        raise ValueError(f"{name}: order {N} outside 2..8")
+    check_zero_fill_value(X)
+    mode = operator.index(mode)
+    if not -N <= mode < N:
+        raise AxisError(mode, N)
+    mode %= N
+    factors = list(factors)
+    if len(factors) != N:
+        raise ValueError(f"{name}: {len(factors)} factors for an order-{N} tensor")
+    others = [m for m in range(N) if m != mode]
+    for m in others:
+        if not D.is_device_tensor(factors[m]):
+            factors[m] = np.asarray(factors[m])
+    return N, mode, factors, others
+
+
 def mttkrp_mode(X, factors, mode):
     """Mode-`mode` MTTKRP of a sparse tensor: the product of the mode-`mode` matricisation of `X` with the Khatri-Rao
     product of every other factor, the step CP-ALS runs once per mode and iteration.
@@ -149,25 +175,7 @@ def mttkrp_mode(X, factors, mode):
     dropped when X's contents are replaced, and are not copied or pickled).  A cached mode holds
     (N * index bytes + value bytes) * nnz of device memory -- index bytes 4 when every extent and nnz fit int32, else 8.
     """
-    from ._gcxs import GCXS
-
-    if not isinstance(X, (COO, GCXS)):
-        raise TypeError("mttkrp_mode: `X` must be a sparse_b200 COO or GCXS array")
-    N = X.ndim
-    if not 2 <= N <= 8:
-        raise ValueError(f"mttkrp_mode: order {N} outside 2..8")
-    check_zero_fill_value(X)
-    mode = operator.index(mode)
-    if not -N <= mode < N:
-        raise AxisError(mode, N)
-    mode %= N
-    factors = list(factors)
-    if len(factors) != N:
-        raise ValueError(f"mttkrp_mode: {len(factors)} factors for an order-{N} tensor")
-    others = [m for m in range(N) if m != mode]
-    for m in others:
-        if not D.is_device_tensor(factors[m]):
-            factors[m] = np.asarray(factors[m])
+    N, mode, factors, others = _tensor_and_factors("mttkrp_mode", X, factors, mode)
     R = int(factors[others[0]].shape[1]) if factors[others[0]].ndim == 2 else -1
     for m in others:
         f = factors[m]
@@ -184,6 +192,56 @@ def mttkrp_mode(X, factors, mode):
         coords, vals = _mode_stream(X, mode)
         fac = [None if m == mode else _dense_dev(factors[m], T) for m in range(N)]
         out = Kn.mttkrp_mode(coords, Kn.cast(vals, T), fac, mode, rows, R)
+    return _return_dense(out, [f for f in factors if f is not None])
+
+
+def ttmc_mode(X, factors, mode):
+    """Mode-`mode` TTMc (tensor times matrix chain) of a sparse tensor: X multiplied by the transpose of every factor but
+    `factors[mode]`, matricised along `mode`, the step HOOI (Tucker decomposition) runs once per mode and iteration.
+
+        out[i, col] = sum over stored entries e with i_mode(e) = i of  v_e * prod_{m != mode} factors[m][i_m(e), r_m]
+
+    `X` is a COO or GCXS of order 2..8 with a zero fill value.  `factors` holds N dense 2-D arrays (NumPy arrays or
+    CUDA tensors), `factors[m]` of shape (X.shape[m], R_m), each mode with its own R_m; `factors[mode]` is never read
+    and may be None.  `mode` counts from the end when negative.  The result is dense, (X.shape[mode], W) with
+    W = prod_{m != mode} R_m, of dtype result_type(X.dtype, other factor dtypes) (float32 or float64): a NumPy array,
+    or a CUDA tensor when a factor is one.
+
+    Columns are in C order over the other modes, ascending: with a < b < ... the modes other than `mode`,
+    col = ((r_a * R_b + r_b) * R_c + r_c) ..., so `out.reshape(X.shape[mode], R_a, R_b, ...)` is
+    `np.einsum` of X with the factors and output subscripts "i" + "abc...".  HOOI takes the leading R_mode left
+    singular vectors of `out`, which do not depend on the column order.  W is at most `_kernels.ttmc_mode_max_width()`
+    (2,097,120: the combine kernel's launch geometry); a larger W raises ValueError before anything is allocated.
+
+    The summation order is fixed (include/sparse_b200.h, b2s_ttmc_mode), so results are reproducible bit for bit.
+    With every R_m = R, the columns (r, r, ..., r) equal `mttkrp_mode`'s column r bit for bit.
+
+    Memory: the result, rows * W * itemsize; the mode stream of `mode`, cached on `X` and shared with `mttkrp_mode`
+    ((N * index bytes + value bytes) * nnz, as described there); and, during the call, a scratch array of
+    2 * ceil(nnz / 512) * W' * itemsize bytes (W' = W rounded up to a multiple of 4) for the rows that cross chunks.
+    """
+    N, mode, factors, others = _tensor_and_factors("ttmc_mode", X, factors, mode)
+    ranks = [0] * N
+    for m in others:
+        f = factors[m]
+        if f.ndim != 2 or int(f.shape[0]) != X.shape[m]:
+            raise ValueError(f"ttmc_mode: shape mismatch X{X.shape}, factor {m} {tuple(f.shape)} "
+                             f"(expected ({X.shape[m]}, R_{m}))")
+        ranks[m] = int(f.shape[1])
+    T = np.result_type(X.dtype, *(_dense_dt(factors[m]) for m in others))
+    if T not in (np.dtype("float32"), np.dtype("float64")):
+        raise TypeError(f"ttmc_mode: dtype {T} is outside the CUDA dtype matrix (float32, float64)")
+    W = int(np.prod([ranks[m] for m in others], dtype=object))
+    if W > Kn.ttmc_mode_max_width():
+        raise ValueError(f"ttmc_mode: {W} output columns (the product of the other modes' ranks) exceed the limit of "
+                         f"{Kn.ttmc_mode_max_width()}")
+    rows = X.shape[mode]
+    if X.nnz == 0 or rows == 0 or W == 0:
+        out = Kn.full(rows * W, 0, T).reshape(rows, W)
+    else:
+        coords, vals = _mode_stream(X, mode)
+        fac = [None if m == mode else _dense_dev(factors[m], T) for m in range(N)]
+        out = Kn.ttmc_mode(coords, Kn.cast(vals, T), fac, mode, rows, ranks)
     return _return_dense(out, [f for f in factors if f is not None])
 
 

@@ -687,6 +687,50 @@ def mttkrp_mode(coords, vals, factors, mode, rows, R):
 
 
 # ------------------------------------------------------------------------------------------------
+# K12 mode-n TTMc
+# ------------------------------------------------------------------------------------------------
+def ttmc_mode_max_width() -> int:
+    """Largest W = prod_{m != mode} R_m that b2s_ttmc_mode accepts (B2S_TTMC_MAX_W, from its launch geometry)."""
+    return int(_lib.load().b2s_ttmc_mode_max_width())
+
+
+def ttmc_mode(coords, vals, factors, mode, rows, ranks):
+    """out[i, col] = sum over the stream entries e with coords[mode][e] = i of vals[e] * prod_{m != mode}
+    factors[m][coords[m][e], r_m], col the C-order index of (r_m for m != mode), in the fixed order of b2s_ttmc_mode.
+    `coords` (N index tensors, one width) and `vals` are the mode stream; `ranks[m]` is factors[m].shape[1];
+    factors[mode] is not read."""
+    t = _t()
+    N = len(coords)
+    dt = D.np_dtype(vals)
+    assert all(c.dtype == coords[0].dtype for c in coords)
+    W = 1
+    for m in range(N):
+        if m != mode:
+            W *= int(ranks[m])
+    fac, ld, keep = [], [], []
+    for m, f in enumerate(factors):
+        if m == mode:
+            fac.append(0)
+            ld.append(0)
+            continue
+        assert f.dtype == vals.dtype
+        R = int(ranks[m])
+        if R > 1 and f.stride(1) != 1:
+            f = f.contiguous()
+        keep.append(f)  # a contiguous copy lives until the launch is enqueued (the caching allocator orders its reuse)
+        fac.append(D.ptr(f))
+        ld.append(f.stride(0) if f.shape[0] > 1 else R)
+    out = t.empty((rows, W), dtype=vals.dtype, device=vals.device)
+    ptrs = (ctypes.c_void_p * N)(*[D.ptr(c) for c in coords])
+    fptrs = (ctypes.c_void_p * N)(*fac)
+    rc = _lib.load().b2s_ttmc_mode(i32(D.dtype_code(dt)), i32(_idx_bytes(coords[0])), i32(N), i32(mode),
+                                   i64(vals.shape[0]), i64(rows), _i64arr([int(r) for r in ranks]), ptrs,
+                                   vp(D.ptr(vals)), fptrs, _i64arr(ld), vp(D.ptr(out)), i64(W), _sp())
+    _lib.check(rc, "b2s_ttmc_mode")
+    return out
+
+
+# ------------------------------------------------------------------------------------------------
 # K11 masked SpGEMM
 # ------------------------------------------------------------------------------------------------
 def masked_spgemm(m_indptr, m_cols, m_vals, a_indptr, a_cols, a_vals, bt_indptr, bt_cols, bt_vals, M, N, K):

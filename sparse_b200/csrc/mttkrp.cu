@@ -296,6 +296,272 @@ static int mttkrp_mode_impl(int order, int mode, int64_t nnz, int64_t rows, int6
     return rc;
 }
 
+// ---------------------------------------------------------------------------------------------------------------------
+// K12: mode-n TTMc (tensor times matrix chain), the Kronecker counterpart of K10.
+//
+//   out[i, col] = sum over stored e with i_n(e) = i of  v_e * U_a[i_a, r_a] * U_b[i_b, r_b] * ... * U_z[i_z, r_z]
+//   col = ((r_a * R_b + r_b) * R_c + r_c) ... (C order over the other modes a < b < ... < z)
+//
+// Same stream, chunks, flush and combine as K10; only the columns differ.  The W = R_a * ... * R_z columns of a row
+// are cut into tiles of G * VEC; lane l of a group owns VEC consecutive columns, which (VEC dividing R_z) share the
+// digits r_a .. r_y.  Per entry the lane gathers the scalars U_a[i_a, r_a] .. U_y[i_y, r_y] (the group reads the same
+// factor rows), forms the prefix ((v * U_a) * ...) * U_y once, and multiplies it by one pack of U_z's row: the
+// association of the order contract, so the vector and scalar forms are bit-identical.  The grid is flat with the column
+// tiles of one chunk range adjacent, so the tiles that re-read a chunk's stream entries run together and mostly find
+// them in L2.
+// ---------------------------------------------------------------------------------------------------------------------
+
+// ranks of the leading other modes (every other mode but the last), ascending
+struct TtmcRanks {
+    int r[kMaxOther];
+};
+
+template <typename T>
+__device__ __forceinline__ T t_stream(const T *p, bool reread) {
+    return reread ? __ldg(p) : ldg_stream(p);  // several column tiles read the stream: keep it in L2 for the others
+}
+
+template <typename T, typename I, int VEC, int G, int U>
+__global__ void __launch_bounds__(256)
+ttmc_mode_kernel(const OtherModes<I> lead, const TtmcRanks rk, const int n_lead, const I *__restrict__ lastc,
+                 const T *__restrict__ fac_last, const int64_t ld_last, const int64_t R_last,
+                 const I *__restrict__ rowc, const T *__restrict__ vals, const int64_t nnz, const int64_t rows,
+                 const int64_t W, const int64_t ntiles, T *__restrict__ out, const int64_t ldo, T *__restrict__ pieces,
+                 const int64_t ldp) {
+    static_assert(G >= 1 && G <= 32 && (G & (G - 1)) == 0, "G must be a power of two <= 32");
+    static_assert(U <= G && G % U == 0, "U must divide G");
+    constexpr unsigned FULL = 0xffffffffu;
+    const int lane = threadIdx.x & 31;
+    const int sub = lane & (G - 1);
+    const int64_t tile = (int64_t)blockIdx.x % ntiles;
+    const int64_t cblock = (int64_t)blockIdx.x / ntiles;
+    const int64_t chunk = (cblock * (blockDim.x >> 5) + (threadIdx.x >> 5)) * (32 / G) + lane / G;
+    const int64_t nchunks = (nnz + kChunk - 1) / kChunk;
+    const int64_t col0 = (tile * G + sub) * VEC;
+    const bool col_ok = col0 < W;
+    const bool reread = ntiles > 1;
+
+    // this lane's digits: r_z0 .. r_z0 + VEC - 1 of the last mode, one digit of each leading mode
+    int64_t q = col_ok ? col0 / R_last : 0;
+    const int64_t rz0 = col_ok ? col0 - q * R_last : 0;
+    int dig[kMaxOther];
+#pragma unroll
+    for (int m = kMaxOther - 1; m >= 0; --m) {
+        dig[m] = 0;
+        if (m < n_lead) {
+            const int64_t qn = q / rk.r[m];
+            dig[m] = (int)(q - qn * rk.r[m]);
+            q = qn;
+        }
+    }
+
+    int64_t base = 0, end = 0, row_first = 0, row_last = 0;
+    bool head_cross = false, tail_cross = false;
+    if (chunk < nchunks) {
+        base = chunk * kChunk;
+        end = base + kChunk < nnz ? base + kChunk : nnz;
+        row_first = (int64_t)rowc[base];
+        row_last = (int64_t)rowc[end - 1];
+        const int64_t prev = chunk > 0 ? (int64_t)rowc[base - 1] : -1;
+        head_cross = prev == row_first;
+        tail_cross = end < nnz && (int64_t)rowc[end] == row_last;
+        if (col_ok) {
+            m_zero_rows<T, VEC>(out, ldo, prev + 1, row_first, col0);
+            if (end == nnz) m_zero_rows<T, VEC>(out, ldo, row_last + 1, rows, col0);
+        }
+    }
+    const uint64_t pol = policy_evict_last();
+
+    T acc[VEC];
+#pragma unroll
+    for (int k = 0; k < VEC; ++k) acc[k] = T(0);
+    int64_t cur = row_first;
+
+    auto flush = [&](int64_t r) {
+        if (!col_ok) return;
+        T *dst;
+        if (r == row_first && (head_cross || (r == row_last && tail_cross))) dst = pieces + (2 * chunk) * ldp + col0;
+        else if (r == row_last && tail_cross) dst = pieces + (2 * chunk + 1) * ldp + col0;
+        else dst = out + r * ldo + col0;
+        m_store<T, VEC>(dst, acc);
+    };
+
+    auto any = [&](bool p) -> bool {
+        if constexpr (G == 32) return p;
+        else return __any_sync(FULL, p);
+    };
+
+    I rc_n = 0, cz_n = 0;
+    I c_n[kMaxOther];
+    T v_n = T(0);
+#pragma unroll
+    for (int m = 0; m < kMaxOther; ++m) c_n[m] = 0;
+    if (base + sub < end) {
+        rc_n = t_stream(rowc + base + sub, reread);
+        v_n = t_stream(vals + base + sub, reread);
+        cz_n = t_stream(lastc + base + sub, reread);
+#pragma unroll
+        for (int m = 0; m < kMaxOther; ++m)
+            if (m < n_lead) c_n[m] = t_stream(lead.coord[m] + base + sub, reread);
+    }
+
+    const T *fz = fac_last + rz0;
+    while (any(base < end)) {
+        const I rc = rc_n, cz = cz_n;
+        const T v = v_n;
+        I c[kMaxOther];
+#pragma unroll
+        for (int m = 0; m < kMaxOther; ++m) c[m] = c_n[m];
+        const int64_t rem = end - base;
+        const int cnt = rem > G ? G : (rem > 0 ? (int)rem : 0);
+        const int64_t nb = base + G;
+        if (nb + sub < end) {
+            rc_n = t_stream(rowc + nb + sub, reread);
+            v_n = t_stream(vals + nb + sub, reread);
+            cz_n = t_stream(lastc + nb + sub, reread);
+#pragma unroll
+            for (int m = 0; m < kMaxOther; ++m)
+                if (m < n_lead) c_n[m] = t_stream(lead.coord[m] + nb + sub, reread);
+        }
+#pragma unroll 1
+        for (int j = 0; j < G; j += U) {
+            if (!any(j < cnt)) break;
+            T pre[U];
+            I rr[U];
+#pragma unroll
+            for (int u = 0; u < U; ++u) {
+                pre[u] = __shfl_sync(FULL, v, j + u, G);
+                rr[u] = __shfl_sync(FULL, rc, j + u, G);
+            }
+            // the prefix ((v * U_a) * U_b) * ... over the leading modes, each product rounded
+#pragma unroll
+            for (int m = 0; m < kMaxOther; ++m) {
+                if (m < n_lead) {
+                    const T *fm = (const T *)lead.fac[m] + dig[m];
+                    const int64_t ldm = lead.ld[m];
+                    T f[U];
+#pragma unroll
+                    for (int u = 0; u < U; ++u) {
+                        const I ix = __shfl_sync(FULL, c[m], j + u, G);
+                        f[u] = j + u < cnt && col_ok ? m_load<T, 1>(fm + (int64_t)ix * ldm, pol).v[0] : T(0);
+                    }
+#pragma unroll
+                    for (int u = 0; u < U; ++u) pre[u] = mul_rn(pre[u], f[u]);
+                }
+            }
+            MPack<T, VEC> f[U];
+#pragma unroll
+            for (int u = 0; u < U; ++u) {
+                const I ix = __shfl_sync(FULL, cz, j + u, G);
+                if (j + u < cnt && col_ok) f[u] = m_load<T, VEC>(fz + (int64_t)ix * ld_last, pol);
+                else {
+#pragma unroll
+                    for (int k = 0; k < VEC; ++k) f[u].v[k] = T(0);
+                }
+            }
+#pragma unroll
+            for (int u = 0; u < U; ++u) {
+                if (j + u < cnt) {
+                    if (rr[u] != cur) {
+                        flush(cur);
+                        if (col_ok) m_zero_rows<T, VEC>(out, ldo, cur + 1, rr[u], col0);
+                        cur = rr[u];
+#pragma unroll
+                        for (int k = 0; k < VEC; ++k) acc[k] = T(0);
+                    }
+#pragma unroll
+                    for (int k = 0; k < VEC; ++k) acc[k] = add_rn(acc[k], mul_rn(pre[u], f[u].v[k]));
+                }
+            }
+        }
+        base = nb;
+    }
+    if (chunk < nchunks) flush(cur);
+}
+
+template <typename T, typename I, int VEC, int G, int U>
+static int launch_ttmc(const OtherModes<I> &lead, const TtmcRanks &rk, int n_lead, const I *lastc, const T *fac_last,
+                       int64_t ld_last, int64_t R_last, const I *rowc, const T *vals, int64_t nnz, int64_t rows,
+                       int64_t W, T *out, int64_t ldo, T *pieces, int64_t ldp, cudaStream_t s) {
+    constexpr int chunks_per_block = 8 * (32 / G);
+    const int64_t nchunks = (nnz + kChunk - 1) / kChunk;
+    const int64_t ntiles = (W + (int64_t)G * VEC - 1) / ((int64_t)G * VEC);
+    const int64_t blocks = (nchunks + chunks_per_block - 1) / chunks_per_block * ntiles;
+    B2S_REQUIRE(blocks <= INT32_MAX, B2S_ERR_INVALID, "ttmc_mode: %lld chunks x %lld column tiles exceed one grid",
+                (long long)nchunks, (long long)ntiles);
+    ttmc_mode_kernel<T, I, VEC, G, U><<<(unsigned)blocks, 256, 0, s>>>(lead, rk, n_lead, lastc, fac_last, ld_last,
+                                                                       R_last, rowc, vals, nnz, rows, W, ntiles, out,
+                                                                       ldo, pieces, ldp);
+    return B2S_OK;
+}
+
+template <typename T, typename I, int VEC>
+static int dispatch_ttmc(const OtherModes<I> &lead, const TtmcRanks &rk, int n_lead, const I *lastc,
+                         const T *fac_last, int64_t ld_last, int64_t R_last, const I *rowc, const T *vals, int64_t nnz,
+                         int64_t rows, int64_t W, T *out, int64_t ldo, T *pieces, int64_t ldp, cudaStream_t s) {
+    const int64_t packs = (W + VEC - 1) / VEC;
+#define B2S_TT(G, U)                                                                                                 \
+    return launch_ttmc<T, I, VEC, G, U>(lead, rk, n_lead, lastc, fac_last, ld_last, R_last, rowc, vals, nnz, rows, W, \
+                                        out, ldo, pieces, ldp, s)
+    // at most 16 lanes per group (two chunks per warp, 16 entries' gathers in flight): against 32 lanes, W = 256 and
+    // 1024 in f32 ran 20 % faster on the H100, more than paying for twice the column tiles
+    if (packs > 8) B2S_TT(16, 8);
+    if (packs > 4) B2S_TT(8, 8);
+    if (packs > 2) B2S_TT(4, 4);
+    if (packs > 1) B2S_TT(2, 2);
+    B2S_TT(1, 1);
+#undef B2S_TT
+}
+
+template <typename T, typename I>
+static int ttmc_mode_impl(int order, int mode, int64_t nnz, int64_t rows, const int64_t *ranks, int64_t W,
+                          const void *const *coords, const void *vals, const void *const *factors, const int64_t *ld,
+                          void *out, int64_t ldo, cudaStream_t s) {
+    constexpr int VEC = 16 / sizeof(T);
+    const int last = mode == order - 1 ? order - 2 : order - 1;
+    OtherModes<I> lead{};
+    TtmcRanks rk{};
+    int n_lead = 0;
+    for (int m = 0; m < last; ++m) {
+        if (m == mode) continue;
+        lead.coord[n_lead] = (const I *)coords[m];
+        lead.fac[n_lead] = factors[m];
+        lead.ld[n_lead] = ld[m];
+        rk.r[n_lead] = (int)ranks[m];
+        ++n_lead;
+    }
+    const int64_t R_last = ranks[last];
+    const bool aligned = R_last % VEC == 0 && ld[last] % VEC == 0 && ((uintptr_t)factors[last] & 15) == 0 &&
+                         ldo % VEC == 0 && ((uintptr_t)out & 15) == 0;
+    const int64_t nchunks = (nnz + kChunk - 1) / kChunk;
+    const int64_t ldp = (W + 3) & ~(int64_t)3;
+    T *pieces = nullptr;
+    int rc = scratch_alloc((void **)&pieces, (size_t)(2 * nchunks * ldp) * sizeof(T), s);
+    if (rc) return rc;
+    const I *rowc = (const I *)coords[mode];
+    const I *lastc = (const I *)coords[last];
+    const T *fl = (const T *)factors[last];
+    if (aligned)
+        rc = dispatch_ttmc<T, I, VEC>(lead, rk, n_lead, lastc, fl, ld[last], R_last, rowc, (const T *)vals, nnz, rows,
+                                      W, (T *)out, ldo, pieces, ldp, s);
+    else
+        rc = dispatch_ttmc<T, I, 1>(lead, rk, n_lead, lastc, fl, ld[last], R_last, rowc, (const T *)vals, nnz, rows, W,
+                                    (T *)out, ldo, pieces, ldp, s);
+    cudaError_t e = cudaGetLastError();
+    if (rc == B2S_OK) count_launch();
+    if (rc == B2S_OK && e == cudaSuccess && nchunks > 1) {
+        const int64_t warps = nchunks - 1;
+        dim3 grid((unsigned)((warps + 7) / 8), (unsigned)((W + 31) / 32));
+        mttkrp_combine_kernel<T, I><<<grid, 256, 0, s>>>(rowc, nnz, W, pieces, ldp, (T *)out, ldo);
+        e = cudaGetLastError();
+        count_launch();
+    }
+    const int frc = scratch_free(pieces, s);
+    if (rc) return rc;
+    B2S_REQUIRE(e == cudaSuccess, B2S_ERR_CUDA, "ttmc_mode: kernel launch failed: %s", cudaGetErrorString(e));
+    return frc;
+}
+
 }  // namespace b2s
 
 using namespace b2s;
@@ -334,6 +600,50 @@ int b2s_mttkrp_mode(int dtype, int idx_bytes, int order, int mode, int64_t nnz, 
     if (idx_bytes == 4) B2S_MI(double, int32_t);
     B2S_MI(double, int64_t);
 #undef B2S_MI
+}
+
+int b2s_ttmc_mode_max_width(void) { return B2S_TTMC_MAX_W; }
+
+int b2s_ttmc_mode(int dtype, int idx_bytes, int order, int mode, int64_t nnz, int64_t rows, const int64_t *ranks_host,
+                  const void *const *coords_host, const void *vals_dev, const void *const *factors_host,
+                  const int64_t *ld_host, void *out_dev, int64_t ldo, void *stream) {
+    B2S_REQUIRE(dtype == B2S_F32 || dtype == B2S_F64, B2S_ERR_UNSUPPORTED, "ttmc_mode: dtype %d (f32/f64 only)", dtype);
+    B2S_REQUIRE(idx_bytes == 4 || idx_bytes == 8, B2S_ERR_INVALID, "ttmc_mode: idx_bytes");
+    B2S_REQUIRE(order >= 2 && order <= 8, B2S_ERR_INVALID, "ttmc_mode: order %d outside 2..8", order);
+    B2S_REQUIRE(mode >= 0 && mode < order, B2S_ERR_INVALID, "ttmc_mode: mode %d of an order-%d tensor", mode, order);
+    B2S_REQUIRE(nnz >= 0 && rows >= 0, B2S_ERR_INVALID, "ttmc_mode: negative size");
+    B2S_REQUIRE(ranks_host != nullptr, B2S_ERR_INVALID, "ttmc_mode: NULL ranks");
+    int64_t W = 1;
+    for (int m = 0; m < order; ++m) {
+        if (m == mode) continue;
+        B2S_REQUIRE(ranks_host[m] >= 0, B2S_ERR_INVALID, "ttmc_mode: negative rank of mode %d", m);
+        if (ranks_host[m] == 0) W = 0;
+        else if (W > 0) W = W > B2S_TTMC_MAX_W / ranks_host[m] ? B2S_TTMC_MAX_W + 1 : W * ranks_host[m];
+    }
+    B2S_REQUIRE(W <= B2S_TTMC_MAX_W, B2S_ERR_INVALID, "ttmc_mode: width above B2S_TTMC_MAX_W = %d", B2S_TTMC_MAX_W);
+    B2S_REQUIRE(ldo >= W, B2S_ERR_INVALID, "ttmc_mode: ldo < W");
+    if (rows == 0 || W == 0) return B2S_OK;
+    B2S_REQUIRE(coords_host != nullptr && factors_host != nullptr && ld_host != nullptr, B2S_ERR_INVALID,
+                "ttmc_mode: NULL pointer array");
+    for (int m = 0; m < order; ++m)
+        B2S_REQUIRE(m == mode || ld_host[m] >= ranks_host[m], B2S_ERR_INVALID, "ttmc_mode: ld of factor %d < R_%d", m,
+                    m);
+    cudaStream_t s = (cudaStream_t)stream;
+    const size_t es = dtype_size(dtype);
+    if (nnz == 0) {
+        B2S_CUDA(cudaMemset2DAsync(out_dev, (size_t)ldo * es, 0, (size_t)W * es, (size_t)rows, s));
+        return B2S_OK;
+    }
+#define B2S_TI(T, I)                                                                                                \
+    return ttmc_mode_impl<T, I>(order, mode, nnz, rows, ranks_host, W, coords_host, vals_dev, factors_host, ld_host, \
+                                out_dev, ldo, s)
+    if (dtype == B2S_F32) {
+        if (idx_bytes == 4) B2S_TI(float, int32_t);
+        B2S_TI(float, int64_t);
+    }
+    if (idx_bytes == 4) B2S_TI(double, int32_t);
+    B2S_TI(double, int64_t);
+#undef B2S_TI
 }
 
 }  // extern "C"

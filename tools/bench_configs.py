@@ -5,9 +5,9 @@ Device-resident inputs (generated with seeded torch generators on the GPU), wall
 torch.cuda.synchronize() because the public calls contain their own size-returning syncs.
 Prints one line per config as it runs and the whole result as one JSON line at the end.
 
-    python tools/bench_configs.py [c1 c3 c3big red c4 c5 mttkrp mttkrp_mode masked]
+    python tools/bench_configs.py [c1 c3 c3big red c4 c5 mttkrp mttkrp_mode masked ttmc]
 
-`masked` (the masked SpGEMM, examples/triangles_example.py) runs only when named.
+`masked` (the masked SpGEMM, examples/triangles_example.py) and `ttmc` (the Tucker / HOOI step) run only when named.
 """
 import json
 import os
@@ -278,6 +278,8 @@ def run(which=None, compact=False, parity=True):
         res.update(_mttkrp_mode_order3(rec, parity))
     if "masked" in which:
         res.update(_masked(rec, parity))
+    if "ttmc" in which:
+        res.update(_ttmc(rec, parity))
     torch.cuda.empty_cache()
     return res
 
@@ -449,6 +451,135 @@ def _mttkrp_mode_order3(rec, parity):
                            "values_close": close, "sampled_rows_bit_exact": bool(exact)}
         out[name] = r
     del X, U, coords, vals
+    return out
+
+
+def _ttmc_parity(X, U, mode, got, ranks, sample_rows, seed):
+    """fp64 device restatement of every row (one block of R_last columns per leading digit, entries in blocks of 1e7)
+    and `sample_rows` rows bit-compared with the CPU restatement of the order (tests/_ttmc_order.py)."""
+    import _ttmc_order as TO
+
+    coords, vals = X._dev()
+    shape, nnz = X.shape, X.nnz
+    a, b = [m for m in range(3) if m != mode]
+    Rb = ranks[b]
+    close = True
+    for ra in range(ranks[a]):
+        want = torch.zeros((shape[mode], Rb), dtype=torch.float64, device=DEV)
+        for s in range(0, nnz, 10_000_000):
+            c = coords[:, s:s + 10_000_000]
+            p = vals[s:s + 10_000_000].double() * U[a][c[a], ra].double()
+            want.index_add_(0, c[mode], p[:, None] * U[b][c[b]].double())
+        close &= bool(torch.allclose(got[:, ra * Rb:(ra + 1) * Rb].double(), want, rtol=2e-5, atol=0))
+        del want
+    exact = True
+    ch = sp._kernels.mttkrp_mode_chunk()
+    for i in np.random.default_rng(seed).choice(shape[mode], sample_rows, replace=False):
+        sel = torch.nonzero(coords[mode] == int(i)).reshape(-1)
+        start = int((coords[mode] < int(i)).sum())
+        c = coords[:, sel]
+        p = TO.products(vals[sel].cpu().numpy(), [U[m][c[m]].cpu().numpy() for m in (a, b)], np.float32)
+        exact &= TO.same_bits(got[int(i)].cpu().numpy(), TO.row_result(p, start, ch, np.float32))
+    return {"vs": f"fp64 device restatement (all rows, rtol 2e-5) + {sample_rows} sampled rows bit-compared with the "
+                  "CPU restatement of the order (tests/_ttmc_order.py)",
+            "values_close": close, "sampled_rows_bit_exact": bool(exact)}
+
+
+def _ttmc_models(X, ranks, mode, vb=4, ib=4):
+    """Byte and op models of one ttmc_mode call from shapes (f32, int32 stream).  Bytes: the stream (N coordinates +
+    value) once per column tile; one full row of every other factor per entry (every gather from HBM: an upper bound,
+    the rows are largely L2 hits); the output; the pieces (written and read back by the combine kernel).  Ops: one
+    multiply and one add per entry and column, plus the prefix multiplies (one per leading mode, per entry and lane)."""
+    N, nnz = X.ndim, X.nnz
+    others = [m for m in range(N) if m != mode]
+    W = int(np.prod([ranks[m] for m in others]))
+    vec = 16 // vb
+    packs = -(-W // vec)
+    G = 16 if packs > 8 else 8 if packs > 4 else 4 if packs > 2 else 2 if packs > 1 else 1  # dispatch_ttmc's groups
+    tiles = -(-W // (G * vec))
+    nchunks = -(-nnz // 512)
+    stream = tiles * nnz * (N * ib + vb)
+    gathers = nnz * sum(ranks[m] for m in others) * vb
+    output = X.shape[mode] * W * vb
+    pieces = 2 * 2 * nchunks * (-(-W // 4) * 4) * vb
+    total = stream + gathers + output + pieces
+    ops = nnz * (2 * W + (len(others) - 1) * packs)
+    sm_ops = 132 * 128 * 1.98e9  # FP32 lanes x the H100 SXM boost clock: separate multiplies and adds per second
+    return {"W": W, "column_tiles": tiles, "bytes": {"stream": stream, "factor_gathers": gathers, "output": output,
+                                                     "pieces": pieces, "total": total},
+            "op_model": ops, "model_ms_bytes_at_3.35TBs": round(total / 3.35e12 * 1e3, 3),
+            "model_ms_ops_at_3.3e13": round(ops / sm_ops * 1e3, 3)}
+
+
+def _ttmc(rec, parity):
+    """Tucker / HOOI step: ttmc_mode on the CP-ALS workload of mttkrp_mode ((1e6, 1e6, 100), nnz 1e8, f32) at R_m = 16
+    (W = 256, every mode) and R_m = 32 (W = 1024, mode 0), and on K9's config at R_m = 8 (W = 64) next to the unfused
+    einsum("ijk,jb,kc->ibc"), whose nnz * W broadcast products are what the fused kernel avoids."""
+    sys.path.insert(0, os.path.join(ROOT, "tests"))
+    out = {}
+    card = _card()
+    shape = (1_000_000, 1_000_000, 100)
+    X = rand_coo(shape, 100_000_000, 61, torch.float32)
+    g = torch.Generator(device=DEV).manual_seed(62)
+    for R, modes in ((16, (0, 1, 2)), (32, (0,))):
+        U = [torch.rand((s, R), generator=g, device=DEV, dtype=torch.float32) for s in shape]
+        for mode in modes:
+            X._mode_streams = None  # first call: builds the mode stream (sort + gathers + narrowing)
+            torch.cuda.synchronize()
+            t0 = time.perf_counter()
+            sp.ttmc_mode(X, U, mode)
+            torch.cuda.synchronize()
+            first = (time.perf_counter() - t0) * 1e3
+            models = _ttmc_models(X, [R] * 3, mode)
+            name = f"ttmc_mode order-3 (1e6,1e6,100) nnz 1e8 R_m={R} (W={R * R}) f32 mode {mode}"
+            r = rec(name, lambda: sp.ttmc_mode(X, U, mode), X.nnz, "Gnnz_s", models["bytes"]["total"])
+            r.update({"card": card, "first_call_ms": round(first, 3), **models})
+            if parity:
+                got = sp.ttmc_mode(X, U, mode)
+                r["parity"] = _ttmc_parity(X, U, mode, got, [R] * 3, 4, 70 + mode)
+                del got
+            out[name] = r
+            torch.cuda.empty_cache()
+        del U
+    del X
+    torch.cuda.empty_cache()
+
+    I_, K_, L_, R = 10_000, 10_000, 1_000, 8
+    Bt = rand_coo((I_, K_, L_), 10_000_000, 31, torch.float32)
+    g = torch.Generator(device=DEV).manual_seed(63)
+    U = [None] + [torch.rand((s, R), generator=g, device=DEV, dtype=torch.float32) for s in (K_, L_)]
+    models = _ttmc_models(Bt, [R] * 3, 0)
+    name = "ttmc_mode K9 config (1e4 x 1e4 x 1e3, nnz 1e7) R_m=8 (W=64) f32 mode 0"
+    r = rec(name, lambda: sp.ttmc_mode(Bt, U, 0), Bt.nnz, "Gnnz_s", models["bytes"]["total"])
+    r.update({"card": card, **models})
+    got = sp.ttmc_mode(Bt, U, 0)
+    if parity:
+        r["parity"] = _ttmc_parity(Bt, U, 0, got, [R] * 3, 4, 73)
+    Uh = [u.cpu().numpy() for u in U[1:]]
+    torch.cuda.synchronize()
+    torch.cuda.reset_peak_memory_stats(DEV)
+    base = torch.cuda.memory_allocated(DEV)
+    unf = {"expression": 'einsum("ijk,jb,kc->ibc", X, U1, U2)', "card": _card()}
+    try:
+        t0 = time.perf_counter()
+        ref = sp.einsum("ijk,jb,kc->ibc", Bt, *Uh)
+        dense = ref.todense_device() if hasattr(ref, "todense_device") else torch.as_tensor(np.asarray(ref)).to(DEV)
+        torch.cuda.synchronize()
+        unf["ms_first"] = round((time.perf_counter() - t0) * 1e3, 3)
+        del ref
+        best, med = timeit(lambda: sp.einsum("ijk,jb,kc->ibc", Bt, *Uh), reps=3, warm=1)
+        unf.update({"ms_best": round(best, 4), "ms_median": round(med, 4), "fits": True,
+                    "peak_extra_bytes": int(torch.cuda.max_memory_allocated(DEV) - base),
+                    "values_close_to_fused": bool(torch.allclose(dense.reshape(I_, R * R), got, rtol=2e-5, atol=1e-6))})
+        r["speedup_vs_unfused"] = round(med / r["ms_median"], 2)
+        del dense
+    except (torch.OutOfMemoryError, RuntimeError) as e:  # the broadcast products do not fit on the card
+        unf.update({"fits": False, "error": str(e).splitlines()[0][:200],
+                    "peak_extra_bytes_before_failure": int(torch.cuda.max_memory_allocated(DEV) - base)})
+    r["unfused"] = unf
+    out[name] = r
+    del Bt, U, got
+    torch.cuda.empty_cache()
     return out
 
 
