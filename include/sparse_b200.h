@@ -109,8 +109,8 @@ int b2s_csr_rows_sorted(int idx_bytes, int64_t M, const void *indptr_dev, const 
 /*
  * K1 with explicit scheduling: n_panels == 1 -> the one-pass kernel; n_panels >= 2 -> tiled passes (one per column
  * tile x K panel, with n_panels K panels) that serve the B-row gathers from L2; n_panels == 0 -> tiled passes when B
- * is larger than twice the L2, nnz >= 64 K and the dtype is fp32 (panel count from the panel budget), the one-pass
- * kernel otherwise.
+ * is larger than twice the L2, nnz >= 48 K and the dtype is fp32 or fp64 (panel count from the panel budget), the
+ * one-pass kernel otherwise.
  * The tiled passes need fp32/fp64 and 16-byte aligned operands (N, ldb, ldc multiples of 16 bytes); other calls take
  * the one-pass kernel.  Rows must be sorted by column for the passes: a device-side check sends a call with any
  * unsorted row to the one-pass kernel, without a host synchronisation.  rows_sorted is advisory (0 = known unsorted,

@@ -81,13 +81,40 @@ panel_offsets_kernel(int64_t M, const I *__restrict__ indptr, const I *__restric
     if (__any_sync(FULL, bad) && lane == 0) atomicOr(unsorted, 1);
 }
 
+// 16-byte B gather straight into r when pred is set; otherwise no request is issued and r keeps its value.  Writing
+// the destination in the load itself (no copy behind it) lets L of these issue back to back into L distinct packs.
+__device__ __forceinline__ void ldg_nc_v4_hint_if(uint4 &r, const void *p, bool pred, uint64_t pol) {
+    asm volatile(
+        "{\n\t.reg .pred q;\n\tsetp.ne.b32 q, %5, 0;\n\t"
+        "@q ld.global.nc.L1::no_allocate.L2::cache_hint.v4.u32 {%0,%1,%2,%3}, [%4], %6;\n\t}"
+        : "+r"(r.x), "+r"(r.y), "+r"(r.z), "+r"(r.w)
+        : "l"(p), "r"((int)pred), "l"(pol));
+}
+
+// One chunk of up to L stored entries of one row of a pass, as one lane of the row's group sees it.
+template <typename T, typename I>
+struct PassChunk {
+    I col;     // column of entry base + sub (0 past the chunk's end)
+    T val;
+    int step;  // the row is row0 + step * stride
+    int info;  // entries in the chunk (0..L) | kHead | kTail | kTouched
+};
+
+// CTAs of 256 threads per SM the register budget is sized for: two (<= 128 registers) while the ring (2L packs of 4
+// registers) leaves room, one for L = 16.  Either way 1024 (L <= 8) or 512 (L = 16) gathers can be in flight per SM.
+constexpr int tile_pass_min_blocks(int L) { return L <= 8 ? 2 : 1; }
+
 // One pass (column tile at col_base, K panel [off_lo, off_hi)).  A group of L lanes owns one row and one tile of L x 16
-// bytes; lane `sub` holds columns col_base + sub*VEC .. +VEC.  Each chunk of L stored entries puts L independent
-// 16-byte B loads in flight per lane (one full line per group at L = 8).  Persistent warps walk rows with a static
-// stride; the next row's first A chunk and the offsets of the row after it are loaded before the current row's gathers,
-// so the offsets -> A -> B -> C chain of a row overlaps the gathers of the previous one.
+// bytes; lane `sub` holds columns col_base + sub*VEC .. +VEC.  Persistent warps walk rows with a static stride; each
+// group walks its own stream of chunks (L stored entries of one row; a row without entries in this panel is one empty
+// chunk, so pass 0 still writes its +0) independently of the other groups of its warp, with no barrier between rows.
+// Software pipeline, one chunk per step, per lane:
+//   * the L gathers of chunk k+1 issue into one half of a two-chunk register ring (2L packs of 16 bytes) before the
+//     FMAs of chunk k consume the other half, so up to 2L gathers are in flight per lane across row boundaries;
+//   * A entries are loaded two chunks ahead of their gathers, the offsets of a row two rows ahead of its A;
+//   * the C partial of a row is loaded right after the previous chunk's FMAs (and its row's store), one step ahead.
 template <typename T, typename I, int L>
-__global__ void __launch_bounds__(256)
+__global__ void __launch_bounds__(256, tile_pass_min_blocks(L))
 spmm_tile_pass_kernel(int64_t M, int64_t N, const T *__restrict__ a_data, const I *__restrict__ a_indices,
                       const I *__restrict__ off_lo, const I *__restrict__ off_hi, const T *__restrict__ B, int64_t ldb,
                       T *__restrict__ C, int64_t ldc, int64_t col_base, int first, int hint,
@@ -96,6 +123,8 @@ spmm_tile_pass_kernel(int64_t M, int64_t N, const T *__restrict__ a_data, const 
     constexpr int VEC = 16 / sizeof(T);
     constexpr int RPW = 32 / L;  // rows per warp
     constexpr unsigned FULL = 0xffffffffu;
+    // chunk info: first / last chunk of its row; the row has entries in this panel
+    constexpr int kHead = 1 << 8, kTail = 2 << 8, kTouched = 4 << 8, kCnt = 0xff;
     const int lane = threadIdx.x & 31;
     const int sub = lane & (L - 1);
     const int grp = lane / L;
@@ -104,86 +133,113 @@ spmm_tile_pass_kernel(int64_t M, int64_t N, const T *__restrict__ a_data, const 
     const int64_t warp0 = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
     const int64_t nwarps = ((int64_t)gridDim.x * blockDim.x) >> 5;
     const int64_t stride = nwarps * RPW;
+    const int64_t row0 = warp0 * RPW + grp;
     const uint64_t pol_b = hint ? policy_evict_last() : policy_evict_normal();
     const T *bcol = B + col0;
+    // a grid has at least 8 warps of at least 2 rows (stride >= 16), so every step used, <= M / 16 + 3, fits an int
+    auto row_of = [&](int step) { return row0 + (int64_t)step * stride; };
+    auto crow = [&](int step) { return C + row_of(step) * ldc + col0; };
 
-    int64_t row = warp0 * RPW + grp;
-    int64_t s = 0, e = 0, sn = 0, en = 0;
-    if (row < M) {
-        s = (int64_t)ldg_stream(off_lo + row);
-        e = (int64_t)ldg_stream(off_hi + row);
-    }
-    if (row + stride < M) {
-        sn = (int64_t)ldg_stream(off_lo + row + stride);
-        en = (int64_t)ldg_stream(off_hi + row + stride);
-    }
-    I colv = 0;
-    T valv = T(0);
-    if (s + sub < e) {
-        colv = ldg_stream(a_indices + s + sub);
-        valv = ldg_stream(a_data + s + sub);
-    }
-    for (int64_t w = warp0; w * RPW < M; w += nwarps, row += stride) {
-        // prefetch: first A chunk of the next row, offsets of the row after it
-        I colv_n = 0;
-        T valv_n = T(0);
-        if (sn + sub < en) {
-            colv_n = ldg_stream(a_indices + sn + sub);
-            valv_n = ldg_stream(a_data + sn + sub);
+    // walker: the next chunk whose A entries are loaded (row row_of(ws), entries [wb, we)), the offsets of the next two
+    // rows, and the info bits of the chunk; rows at or past M are empty
+    auto offsets = [&](int step, I &s, I &e) {
+        const int64_t r = row_of(step);
+        s = e = 0;
+        if (r < M) {
+            s = ldg_stream(off_lo + r);
+            e = ldg_stream(off_hi + r);
         }
-        int64_t s2 = 0, e2 = 0;
-        if (row + 2 * stride < M) {
-            s2 = (int64_t)ldg_stream(off_lo + row + 2 * stride);
-            e2 = (int64_t)ldg_stream(off_hi + row + 2 * stride);
+    };
+    int ws = 0;
+    I wb, we, ns, ne, n2s, n2e;
+    offsets(0, wb, we);
+    offsets(1, ns, ne);
+    offsets(2, n2s, n2e);
+    int wflags = kHead | (wb < we ? kTouched : 0);
+    auto next_chunk = [&]() {
+        PassChunk<T, I> c;
+        const int64_t rem = (int64_t)we - (int64_t)wb;
+        c.step = ws;
+        c.info = wflags | (rem > L ? L : (rem > 0 ? (int)rem : 0)) | (rem > L ? 0 : kTail);
+        c.col = 0;
+        c.val = T(0);
+        if (sub < rem) {
+            c.col = ldg_stream(a_indices + (int64_t)wb + sub);
+            c.val = ldg_stream(a_data + (int64_t)wb + sub);
         }
-        const bool row_ok = row < M;
-        T *crow = C + row * ldc + col0;
-        PPack<T, VEC> acc;
+        if (rem > L) {
+            wb += L;
+            wflags = kTouched;
+        } else {
+            ++ws;
+            wb = ns;
+            we = ne;
+            ns = n2s;
+            ne = n2e;
+            offsets(ws + 2, n2s, n2e);
+            wflags = kHead | (wb < we ? kTouched : 0);
+        }
+        return c;
+    };
+
+    // a step whose chunks are all empty (rows without entries in this panel) skips the shuffles, gathers and FMAs
+    auto issue = [&](uint4(&ring)[L], const PassChunk<T, I> &c) {
+        if (!__any_sync(FULL, c.info & kCnt)) return;
 #pragma unroll
-        for (int k = 0; k < VEC; ++k) acc.v[k] = T(0);
-        if (!first && s < e && col_ok) {
-            const uint4 u = ldg_cs_v4(crow);
-            memcpy(&acc, &u, 16);
+        for (int u = 0; u < L; ++u) {
+            const I cu = __shfl_sync(FULL, c.col, u, L);
+            ldg_nc_v4_hint_if(ring[u], bcol + (int64_t)cu * ldb, u < (c.info & kCnt) && col_ok, pol_b);
         }
-        for (int64_t base = s; __any_sync(FULL, base < e); base += L) {
-            const I col = colv;
-            const T val = valv;
-            const int64_t rem = e - base;
-            const int cnt = rem > L ? L : (rem > 0 ? (int)rem : 0);
-            if (base + L + sub < e) {  // next chunk of this row while this one is consumed
-                colv = ldg_stream(a_indices + base + L + sub);
-                valv = ldg_stream(a_data + base + L + sub);
-            }
-            PPack<T, VEC> bv[L];
+    };
+    uint4 part = make_uint4(0, 0, 0, 0);  // C partial of the next chunk's row (later passes)
+    auto load_partial = [&](const PassChunk<T, I> &c) {
+        if ((c.info & kHead) && !first && (c.info & kTouched) && col_ok) part = ldg_cs_v4(crow(c.step));
+    };
+    PPack<T, VEC> acc;
+    auto consume = [&](const uint4(&ring)[L], const PassChunk<T, I> &c) {
+        if (c.info & kHead) {
+            const uint4 a0 = (!first && (c.info & kTouched) && col_ok) ? part : make_uint4(0, 0, 0, 0);
+            memcpy(&acc, &a0, 16);
+        }
+        if (__any_sync(FULL, c.info & kCnt)) {
 #pragma unroll
             for (int u = 0; u < L; ++u) {
-                const I c = __shfl_sync(FULL, col, u, L);
-                if (u < cnt && col_ok) {
-                    const uint4 raw = ldg_nc_v4_hint(bcol + (int64_t)c * ldb, pol_b);
-                    memcpy(&bv[u], &raw, 16);
-                }
-            }
+                const T v = __shfl_sync(FULL, c.val, u, L);
+                if (u < (c.info & kCnt)) {
+                    PPack<T, VEC> b;
+                    memcpy(&b, &ring[u], 16);
 #pragma unroll
-            for (int u = 0; u < L; ++u) {
-                const T v = __shfl_sync(FULL, val, u, L);
-                if (u < cnt) {
-#pragma unroll
-                    for (int k = 0; k < VEC; ++k) acc.v[k] = add_rn(acc.v[k], mul_rn(v, bv[u].v[k]));
+                    for (int k = 0; k < VEC; ++k) acc.v[k] = add_rn(acc.v[k], mul_rn(v, b.v[k]));
                 }
             }
         }
         // pass 0 writes every row (rows without entries get +0, as in K1); later passes only rows they touched
-        if (row_ok && col_ok && (first || s < e)) {
+        if ((c.info & kTail) && row_of(c.step) < M && col_ok && (first || (c.info & kTouched))) {
             uint4 u;
             memcpy(&u, &acc, 16);
-            stg_cs_v4(crow, u);
+            stg_cs_v4(crow(c.step), u);
         }
-        s = sn;
-        e = en;
-        sn = s2;
-        en = e2;
-        colv = colv_n;
-        valv = valv_n;
+    };
+
+    uint4 ring0[L], ring1[L];
+#pragma unroll
+    for (int u = 0; u < L; ++u) ring0[u] = ring1[u] = make_uint4(0, 0, 0, 0);
+    PassChunk<T, I> c0 = next_chunk(), c1 = next_chunk(), c2 = next_chunk();
+    // one step: c0's gathers are in `cur`; c1's go into `nxt`
+    auto step = [&](const uint4(&cur)[L], uint4(&nxt)[L]) {
+        if (!__any_sync(FULL, row_of(c0.step) < M)) return false;
+        issue(nxt, c1);
+        const PassChunk<T, I> c3 = next_chunk();
+        consume(cur, c0);
+        load_partial(c1);
+        c0 = c1;
+        c1 = c2;
+        c2 = c3;
+        return true;
+    };
+    issue(ring0, c0);
+    load_partial(c0);
+    while (step(ring0, ring1) && step(ring1, ring0)) {
     }
 }
 
@@ -220,17 +276,18 @@ __global__ void max_row_kernel(int64_t M, const I *__restrict__ indptr, unsigned
 // ---------------------------------------------------------------------------
 // selection and host-side driver
 // ---------------------------------------------------------------------------
-// Defaults from tools/tune_panels.py on an H100 80GB HBM3 at 700 W (one-pass kernel 16.65 ms at C2 in the same run):
-// C2 with 128-byte tiles takes 13.50 / 12.28 / 11.86 / 12.90 / 14.14 ms at 12 / 16 / 24 / 32 / 48 MB per pass; 64-byte
-// tiles are never faster than 16.7 ms (the A stream is read once per tile) and 256-byte tiles not faster than 13.2 ms
-// (twice the panels for the same L2 footprint).  With every column inside one 16 MB panel (all gathers L2 hits) the
-// passes take 9.82 ms: the L2 line rate, not DRAM, is now the limit.  The passes carry a fixed cost (C read and
-// written 2P-1 times, offsets), so they lose at low reuse: 3.76 vs 1.87 ms at nnz / K = 10, 5.98 vs 5.22 ms at 30.
-// They did not gain for fp64 (N = 64: 17.89 vs 17.85 ms), so the automatic choice is fp32 only.
+// Defaults from tools/tune_panels.py on an H100 80GB HBM3 at 700 W (one-pass kernel 16.19 ms at C2 in the same run).
+// C2 with 128-byte tiles: 14.89 / 12.34 / 10.90 / 10.17 / 10.03 / 10.94 ms at 8 / 12 / 16 / 24 / 32 / 48 MB per pass
+// (24 MB kept: at a 400 W limit 24 MB gave 12.4-12.8 ms and 32 MB 13.7-14.4 ms over two runs); 64-byte tiles never
+// below 20.8 ms (A is read once per tile, and a 4-entry chunk carries the same per-step cost), 256-byte tiles not below
+// 12.86 ms.  With every column inside one 16 MB panel (all gathers after the first touch are L2 hits) the passes take
+// 9.44 ms = 42 G line-gathers/s, 7 % below C2: the L2 line rate is the limit.  Forced passes vs the one-pass kernel
+// around the thresholds: nnz / K = 10: 4.08 vs 1.81 ms, 30: 5.45 vs 5.08, 50: 7.04 vs 8.30, 70: 8.34 vs 11.48; K = 1e5
+// (B about one L2): 1.54 vs 1.22 ms at nnz / K = 100, 2.95 vs 2.68 at 300; fp64 N = 64: 11.45 vs 17.17 ms.
 constexpr int64_t kPanelBytes = 24ll << 20;  // B bytes (one panel x one tile) per pass
 constexpr int kTileBytes = 128;               // column tile: one cache line per gather
 constexpr int kL2Multiple = 2;                // tiled only when B is larger than this many L2s ...
-constexpr int64_t kMinReuse = 64;             // ... and each B row is used at least this often (nnz / K)
+constexpr int64_t kMinReuse = 48;             // ... and each B row is used at least this often (nnz / K)
 
 static int64_t g_panel_bytes = 0;  // b2s_spmm_set_tiling (0 = default)
 static int g_tile_bytes = 0;
@@ -263,7 +320,7 @@ static int choose_panels(int dtype, int64_t K, int64_t N, int64_t nnz, bool vec_
                          int rows_sorted) {
     if ((dtype != B2S_F32 && dtype != B2S_F64) || !vec_ok || rows_sorted == 0) return 0;
     if (n_panels >= 2) return n_panels;
-    if (n_panels != 0 || long_rows || nnz < 0 || K <= 0 || dtype != B2S_F32) return 0;
+    if (n_panels != 0 || long_rows || nnz < 0 || K <= 0) return 0;
     const size_t es = dtype_size(dtype);
     if (K * N * (int64_t)es <= kL2Multiple * l2_bytes() || nnz < kMinReuse * K) return 0;
     const int64_t slice_row = (int64_t)tile_lanes(N, es) * 16;  // B bytes of one row within one tile
@@ -394,7 +451,7 @@ int b2s_spmm_set_tiling(int64_t panel_bytes, int tile_bytes) {
 /*
  * K1 with explicit scheduling control.  n_panels == 1: the one-pass kernel.  n_panels >= 2: tiled passes with that many
  * K panels (fp32/fp64 with 16-byte aligned operands; otherwise the one-pass kernel).  n_panels == 0: tiled passes for
- * fp32 when B is larger than kL2Multiple L2s and nnz >= kMinReuse x K (P from the panel budget), else the one-pass
+ * fp32/fp64 when B is larger than kL2Multiple L2s and nnz >= kMinReuse x K (P from the panel budget), else the one-pass
  * kernel.
  * rows_sorted is advisory (0 = known unsorted: skip the passes); the passes check the order on the device themselves.
  */

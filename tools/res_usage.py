@@ -13,7 +13,7 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 LIB = os.path.join(ROOT, "sparse_b200", "libsparse_b200.so")
 # the instantiations the benchmark configurations launch (fp32 / fp64 values, int32 / int64 indices)
 HOT = [r"spmm_csr_dense_dyn_kernel<float, int, 4, 32, 8, 4>", r"spmm_csr_dense_dyn_kernel<float, int, 4, 32, 8, 5>",
-       r"spmm_csr_dense_kernel<float, int, 4, 32, 8",
+       r"spmm_csr_dense_kernel<float, int, 4, 32, 8", r"spmm_tile_pass_kernel<float, int, 8>",
        r"spmm_long_rows_ring_kernel<float", r"spgemm_products_kernel", r"spgemm_rows_kernel<float",
        r"spgemm_rows_kernel<double", r"spgemm_block_kernel<float", r"spgemm_finish_kernel<float",
        r"ew_merge_kernel<double", r"ew_merge_kernel<float", r"rd_count_kernel", r"rd_emit_kernel<double",

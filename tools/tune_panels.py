@@ -3,7 +3,8 @@
 
 At C2 (CSR 1e6 x 1e6, nnz 1e8, B 1e6 x 128 fp32): panel budgets x tile widths, the all-hit ceiling (same shape and nnz,
 every column inside one 16 MB panel, so every gather after the first touch of a line is an L2 hit), evict_last
-against no L2 hint on the B loads, and shapes on both sides of the automatic choice.  Every timed result is compared
+against no L2 hint on the B loads, and shapes on both sides of the automatic choice (one-pass, automatic, and the
+passes forced at the default panel budget).  Every timed result is compared
 bit for bit with the one-pass kernel.  Next to each time: the DRAM-byte model of the path (computed from shapes, not
 measured).  Run from the repository root: python tools/tune_panels.py
 """
@@ -142,10 +143,14 @@ def main():
         ta = timeit(fa)
         es = torch.finfo(dt).bits // 8
         n_l = launches(fa)
+        eq = bool(torch.equal(Cn, rr))
         P, tbe = panels_of(k, n, es, 24 * MB, 128)
+        # the passes forced at the default panel budget (at least 2 panels), whichever side of the thresholds
+        tt = timeit(run(v, c, p, Bn, m, k, n, Cn, max(2, P)))
         shapes.append({"M": m, "K": k, "nnz": int(v.numel()), "N": n, "dtype": str(dt).replace("torch.", ""),
                        "one_pass_ms": round(t1, 3), "auto_ms": round(ta, 3), "auto_launches": n_l,
-                       "auto_is_tiled": n_l > 3, "bit_equal": bool(torch.equal(Cn, rr)),
+                       "auto_is_tiled": n_l > 3, "tiled_ms": round(tt, 3), "tiled_P": max(2, P),
+                       "bit_equal": eq and bool(torch.equal(Cn, rr)),
                        "gather_model_GB": round(bench.algorithmic_bytes(int(v.numel()), m, n) * es / 4 / 1e9, 2),
                        "tiled_dram_model_GB": dram_model(m, k, n, int(v.numel()), es, 4, tbe, P)["total_GB"]})
         print(shapes[-1], file=sys.stderr, flush=True)
