@@ -345,6 +345,27 @@ int b2s_ttmc_mode(int dtype, int idx_bytes, int order, int mode, int64_t nnz, in
                   const void *const *coords_host, const void *vals_dev, const void *const *factors_host,
                   const int64_t *ld_host, void *out_dev, int64_t ldo, void *stream);
 
+/* ---- a sparse tensor of order 2..8 times a CP model at its stored entries (K13, tttp.cu; TTTP, the order-N SDDMM,
+ * no reference counterpart) ------------------------------------------------------------------------------------------
+ * out_vals[e] = v_e * sum_r U_0[i_0(e), r] * U_1[i_1(e), r] * ... * U_{order-1}[i_{order-1}(e), r] for each of the nnz
+ * entries e, in the order they are given: coords_host[m] (m < order) are device pointers to the entries' coordinate
+ * arrays (idx_bytes wide), vals_dev their values; factors_host[m] / ld_host[m] (row stride in elements, >= R) are the
+ * R-column factor matrices, every one read (they may be NULL when R = 0).  No sort, no atomics, no scratch memory, no
+ * stream synchronisation.
+ *
+ * Fixed order of operations (results are reproducible bit for bit, whatever the grid, SM count, index width, stream or
+ * column path):
+ *  1. q_r = ((U_0[i_0, r] * U_1[i_1, r]) * U_2[i_2, r]) * ... * U_{order-1}[i_{order-1}, r], in ascending mode order,
+ *     each product rounded separately; no FMA contraction.
+ *  2. m = ((+0 + q_0) + q_1) + ... + q_{R-1}, in ascending r, each sum rounded; m = +0 when R = 0.
+ *  3. out_vals[e] = v_e * m, one rounding.
+ * Folding CP weights lam into the first factor (U_0[i, r] * lam_r) gives the same bits as a kernel that starts each
+ * product of step 1 with lam_r, ((lam_r * U_0[i_0, r]) * U_1[i_1, r]) * ..., since a rounded product commutes.
+ */
+int b2s_tttp(int dtype, int idx_bytes, int order, int64_t nnz, int64_t R, const void *const *coords_host,
+             const void *vals_dev, const void *const *factors_host, const int64_t *ld_host, void *out_vals_dev,
+             void *stream);
+
 /* ---- masked sparse x sparse product (K11, masked_spgemm.cu; examples/triangles_example.py) ------------------------
  * out_vals[p] = value of mask * (A @ B) at every stored mask entry p, given the mask as CSR (m_indptr over the M rows,
  * m_cols, m_vals already in the output dtype `dtype_out`), A as CSR (M x K) and B^T as CSR (N x K, i.e. B by

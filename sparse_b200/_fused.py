@@ -9,7 +9,8 @@ BLAS / reduceat order, so parity is tolerance-based (rtol 1e-5 f32, 1e-12 f64 in
 
 mttkrp_mode(X, factors, mode) generalises mttkrp to any mode of a tensor of order 2..8 (the CP-ALS step); it has no
 counterpart in the reference beyond the unfused broadcast expression / einsum.  ttmc_mode(X, factors, mode) is its
-Kronecker counterpart, the TTMc step of Tucker / HOOI, with the same inputs and a rank per mode.
+Kronecker counterpart, the TTMc step of Tucker / HOOI, with the same inputs and a rank per mode.  tttp(X, factors)
+evaluates a CP model at X's stored entries (X * [[U_0, ..., U_{N-1}]], the order-N sddmm) and keeps X's pattern.
 
 masked_matmul(mask, a, b) == mask * (a @ b) at mask's stored positions, for sparse a and b: the masked SpGEMM of
 examples/triangles_example.py (sum(a @ a * a) / 6) and of the GraphBLAS masked mxm.  It never forms the product
@@ -132,8 +133,8 @@ def _mode_stream(X, mode):
 
 
 def _tensor_and_factors(name, X, factors, mode):
-    """Checks shared by mttkrp_mode and ttmc_mode: (order N, mode in 0..N-1, the factors as a list with the other
-    modes' ones as NumPy arrays or device tensors, the other modes ascending)."""
+    """Checks shared by mttkrp_mode, ttmc_mode and tttp: (order N, mode in 0..N-1, the factors as a list with the other
+    modes' ones as NumPy arrays or device tensors, the other modes ascending).  `mode` None (tttp) reads every factor."""
     from ._gcxs import GCXS
 
     if not isinstance(X, (COO, GCXS)):
@@ -142,10 +143,11 @@ def _tensor_and_factors(name, X, factors, mode):
     if not 2 <= N <= 8:
         raise ValueError(f"{name}: order {N} outside 2..8")
     check_zero_fill_value(X)
-    mode = operator.index(mode)
-    if not -N <= mode < N:
-        raise AxisError(mode, N)
-    mode %= N
+    if mode is not None:
+        mode = operator.index(mode)
+        if not -N <= mode < N:
+            raise AxisError(mode, N)
+        mode %= N
     factors = list(factors)
     if len(factors) != N:
         raise ValueError(f"{name}: {len(factors)} factors for an order-{N} tensor")
@@ -243,6 +245,83 @@ def ttmc_mode(X, factors, mode):
         fac = [None if m == mode else _dense_dev(factors[m], T) for m in range(N)]
         out = Kn.ttmc_mode(coords, Kn.cast(vals, T), fac, mode, rows, ranks)
     return _return_dense(out, [f for f in factors if f is not None])
+
+
+def _gcxs_coords(X, limit):
+    """Per-axis coordinates of a GCXS's entries in its stored order: the compressed row of each entry from `indptr`,
+    the row and `indices` unravelled over the compressed and the other axes, put back in axis order.  No sort."""
+    _, indices, indptr = X._dev()
+    idt = np.int32 if limit < 2**31 - 1 else np.int64
+    rs, k = X._reordered_shape, X._axisptr
+    lead = Kn.unravel(Kn.rows_from_indptr(indptr, X.nnz, np.int64), rs[:k], idt)
+    rest = Kn.unravel(Kn.cast(indices, np.int64), rs[k:], idt)
+    coords = [None] * X.ndim
+    for pos, a in enumerate(X._axis_order):
+        coords[a] = lead[pos] if pos < k else rest[pos - k]
+    return coords
+
+
+def tttp(X, factors):
+    """A sparse tensor times a CP (Kruskal) model at its stored entries, ``X * [[U_0, ..., U_{N-1}]]`` (TTTP, the
+    order-N SDDMM): the model's residual, loss derivative or ratio at the observed entries that tensor completion, GCP
+    and CP-APR need, without forming the dense model or the nnz x R broadcast products.
+
+        z_e = v_e * sum_r  U_0[i_0(e), r] * U_1[i_1(e), r] * ... * U_{N-1}[i_{N-1}(e), r]
+
+    `X` is a COO or GCXS of order 2..8 with a zero fill value.  `factors` holds N dense 2-D arrays (NumPy arrays or CUDA
+    tensors, which may be mixed), `factors[m]` of shape (X.shape[m], R) with one R for all (R = 0 gives v_e * +0); every
+    factor is read.  The result has X's format and shape (a GCXS keeps ``X.compressed_axes``), dtype
+    result_type(X.dtype, factor dtypes) (float32 or float64) and fill value +0.  It stores X's entries except those
+    whose z_e is bitwise +0; stored -0.0 and NaN results stay (the prune rule of `sddmm` and `masked_matmul`).  At order
+    2 it equals ``sddmm(X, U_0, U_1, b_transposed=True)`` to rounding (K8 sums in another order).
+
+    The order of operations is fixed (include/sparse_b200.h, b2s_tttp): for each r the product in ascending mode order,
+    the sum over r ascending from +0, then one multiply by v_e; results are reproducible bit for bit.  With that order,
+    CP weights lam fold into the first factor: ``tttp(X, [U_0 * lam, U_1, ...])`` has the bits of a kernel that starts
+    each product with lam_r, ((lam_r * U_0) * U_1) * ..., so there is no weights argument.
+
+    One difference from the unfused ``X * model``: its fill value is ``0 * model[0, ..., 0]``, which is -0.0 when that
+    corner of the model is negative; tttp always returns +0, as `masked_matmul` does.
+
+    Entries are taken in place, with no sort: a COO in its canonical order (the mode-0 stream that `mttkrp_mode` also
+    uses and caches), a GCXS in its stored order, and the GCXS result shares X's index arrays unless entries are pruned.
+    A GCXS whose rows repeat an index gets one product per stored entry.  Memory: the result values, plus N coordinate
+    arrays of nnz entries for a GCXS during the call.
+    """
+    from ._gcxs import GCXS
+
+    given = list(factors)
+    N, _, factors, _ = _tensor_and_factors("tttp", X, given, None)
+    for m in range(N):
+        if given[m] is None:
+            raise ValueError(f"tttp: factor {m} is None (tttp reads every factor)")
+    R = int(factors[0].shape[1]) if factors[0].ndim == 2 else -1
+    for m, f in enumerate(factors):
+        if f.ndim != 2 or int(f.shape[0]) != X.shape[m] or int(f.shape[1]) != R:
+            raise ValueError(f"tttp: shape mismatch X{X.shape}, factor {m} {tuple(f.shape)} "
+                             f"(expected ({X.shape[m]}, R) with one R for all factors)")
+    T = np.result_type(X.dtype, *(_dense_dt(f) for f in factors))
+    if T not in (np.dtype("float32"), np.dtype("float64")):
+        raise TypeError(f"tttp: dtype {T} is outside the CUDA dtype matrix (float32, float64)")
+    limit = 2**63 if _FORCE_WIDE_INDEX else max(*X.shape, X.nnz)
+    if isinstance(X, GCXS):
+        data, indices, indptr = X._dev()
+        if X.nnz == 0:
+            out = Kn.full(0, 0, T)
+        else:
+            out = Kn.tttp(_gcxs_coords(X, limit), Kn.cast(data, T), [_dense_dev(f, T) for f in factors], R)
+        res = GCXS._from_device(out, indices, indptr, X.shape, X.compressed_axes, T.type(0))
+        res._idx_vis = X._idx_vis
+        res._prune()  # drops results that are bitwise +0, as X * model does
+        return res
+    if X.nnz == 0:
+        out = Kn.full(0, 0, T)
+    else:
+        coords, vals = _mode_stream(X, 0)
+        out = Kn.tttp(coords, Kn.cast(vals, T), [_dense_dev(f, T) for f in factors], R)
+    res = COO._from_device(X._dev()[0], out, X.shape, T.type(0), keys=X._keys)
+    res._canonicalise(check_sort=False, sum_dups=False, prune=True)  # drops bitwise +0 results, as X * model does
+    return res
 
 
 # Test hook: True keeps masked_matmul's index arrays int64 even when every extent and nnz fit int32.

@@ -731,6 +731,33 @@ def ttmc_mode(coords, vals, factors, mode, rows, ranks):
 
 
 # ------------------------------------------------------------------------------------------------
+# K13 TTTP
+# ------------------------------------------------------------------------------------------------
+def tttp(coords, vals, factors, R):
+    """out[e] = vals[e] * sum_r prod_m factors[m][coords[m][e], r], in the fixed order of b2s_tttp.  `coords` (N index
+    tensors, one width) and `vals` give the entries in the order of the result; every factor is read."""
+    t = _t()
+    N = len(coords)
+    dt = D.np_dtype(vals)
+    assert all(c.dtype == coords[0].dtype for c in coords)
+    fac, ld, keep = [], [], []
+    for f in factors:
+        assert f.dtype == vals.dtype
+        if R > 1 and f.stride(1) != 1:
+            f = f.contiguous()
+        keep.append(f)  # a contiguous copy lives until the launch is enqueued (the caching allocator orders its reuse)
+        fac.append(D.ptr(f))
+        ld.append(f.stride(0) if f.shape[0] > 1 else R)
+    out = t.empty_like(vals)
+    ptrs = (ctypes.c_void_p * N)(*[D.ptr(c) for c in coords])
+    fptrs = (ctypes.c_void_p * N)(*fac)
+    rc = _lib.load().b2s_tttp(i32(D.dtype_code(dt)), i32(_idx_bytes(coords[0])), i32(N), i64(vals.shape[0]), i64(R),
+                              ptrs, vp(D.ptr(vals)), fptrs, _i64arr(ld), vp(D.ptr(out)), _sp())
+    _lib.check(rc, "b2s_tttp")
+    return out
+
+
+# ------------------------------------------------------------------------------------------------
 # K11 masked SpGEMM
 # ------------------------------------------------------------------------------------------------
 def masked_spgemm(m_indptr, m_cols, m_vals, a_indptr, a_cols, a_vals, bt_indptr, bt_cols, bt_vals, M, N, K):

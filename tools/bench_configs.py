@@ -5,9 +5,10 @@ Device-resident inputs (generated with seeded torch generators on the GPU), wall
 torch.cuda.synchronize() because the public calls contain their own size-returning syncs.
 Prints one line per config as it runs and the whole result as one JSON line at the end.
 
-    python tools/bench_configs.py [c1 c3 c3big red c4 c5 mttkrp mttkrp_mode masked ttmc]
+    python tools/bench_configs.py [c1 c3 c3big red c4 c5 mttkrp mttkrp_mode masked ttmc tttp]
 
-`masked` (the masked SpGEMM, examples/triangles_example.py) and `ttmc` (the Tucker / HOOI step) run only when named.
+`masked` (the masked SpGEMM, examples/triangles_example.py), `ttmc` (the Tucker / HOOI step) and `tttp` (a CP model at
+a sparse tensor's entries) run only when named.
 """
 import json
 import os
@@ -280,6 +281,8 @@ def run(which=None, compact=False, parity=True):
         res.update(_masked(rec, parity))
     if "ttmc" in which:
         res.update(_ttmc(rec, parity))
+    if "tttp" in which:
+        res.update(_tttp(rec, parity))
     torch.cuda.empty_cache()
     return res
 
@@ -579,6 +582,147 @@ def _ttmc(rec, parity):
     r["unfused"] = unf
     out[name] = r
     del Bt, U, got
+    torch.cuda.empty_cache()
+    return out
+
+
+def _tttp_parity(X, U, got, samples, seed):
+    """Every entry against an fp64 device restatement (rtol 2e-5) and `samples` sampled entries bit-compared with the
+    CPU restatement of the order (tests/_tttp_order.py).  X is COO; `got` has X's pattern (nothing pruned)."""
+    import _tttp_order as TP
+
+    coords, vals = X._dev()
+    gv = got._data_dev()
+    close = got.nnz == X.nnz
+    for s in range(0, X.nnz, 10_000_000):
+        c = coords[:, s:s + 10_000_000]
+        m = U[0][c[0]].double()
+        for k in range(1, X.ndim):
+            m = m * U[k][c[k]].double()
+        close &= bool(torch.allclose(gv[s:s + 10_000_000].double(), vals[s:s + 10_000_000].double() * m.sum(1),
+                                     rtol=2e-5, atol=0))
+        del m
+    pick = torch.from_numpy(np.sort(np.random.default_rng(seed).choice(X.nnz, samples, replace=False))).to(DEV)
+    want = TP.values(coords[:, pick].cpu().numpy(), vals[pick].cpu().numpy(), [u.cpu().numpy() for u in U],
+                     np.float32)
+    return {"vs": f"fp64 device restatement (all entries, rtol 2e-5) + {samples} sampled entries bit-compared with the "
+                  "CPU restatement of the order (tests/_tttp_order.py)",
+            "values_close": close, "sampled_entries_bit_exact": TP.same_bits(gv[pick].cpu().numpy(), want)}
+
+
+def _tttp_models(X, R, vb=4, ib=4):
+    """Byte model of one tttp call from shapes (f32, int32 coordinates): the entry stream, the output values, and one
+    R-column row of every factor per entry counted as if every gather came from HBM (most are L2 hits, so the kernel
+    may beat this model; it is not an HBM share)."""
+    N, nnz = X.ndim, X.nnz
+    b = {"stream": nnz * (N * ib + vb), "output": nnz * vb, "factor_gathers": nnz * N * R * vb}
+    b["total"] = sum(b.values())
+    return {"bytes": b, "model_ms_bytes_at_3.35TBs": round(b["total"] / 3.35e12 * 1e3, 3)}
+
+
+def _no_zero_values(X):
+    """X with 0.1 added to every value: tttp of a positive model then prunes nothing, so results align with X."""
+    coords, vals = X._dev()
+    return sp.COO(coords, vals + 0.1, shape=X.shape, has_duplicates=False, sorted=True)
+
+
+def _tttp(rec, parity):
+    """CP model at the stored entries: tttp on the CP-ALS workload of mttkrp_mode ((1e6, 1e6, 100), nnz 1e8, R = 32,
+    f32, COO and one GCXS layout); at order 2 on C4's shape next to sddmm, alternating; and on K9's config next to the
+    unfused einsum("ijk,ir,jr,kr->ijk"), whose nnz * R products are what the fused kernel avoids."""
+    sys.path.insert(0, os.path.join(ROOT, "tests"))
+    import _tttp_order as TP
+
+    out = {}
+    card = _card()
+    shape, R = (1_000_000, 1_000_000, 100), 32
+    X = _no_zero_values(rand_coo(shape, 100_000_000, 81, torch.float32))
+    g = torch.Generator(device=DEV).manual_seed(82)
+    U = [torch.rand((s, R), generator=g, device=DEV, dtype=torch.float32) + 0.05 for s in shape]
+    models = _tttp_models(X, R)
+    name = "tttp order-3 (1e6,1e6,100) nnz 1e8 R=32 f32 COO"
+    r = rec(name, lambda: sp.tttp(X, U), X.nnz, "Gnnz_s", models["bytes"]["total"])
+    r.update({"card": card, **models})
+    if parity:
+        got = sp.tttp(X, U)
+        r["parity"] = _tttp_parity(X, U, got, 10_000, 83)
+        del got
+    out[name] = r
+    G = X.asformat("gcxs", compressed_axes=(2,))
+    name = "tttp order-3 (1e6,1e6,100) nnz 1e8 R=32 f32 GCXS compressed_axes=(2,)"
+    r = rec(name, lambda: sp.tttp(G, U), X.nnz, "Gnnz_s")
+    r["card"] = card
+    if parity:
+        gc = sp.tttp(G, U).tocoo()
+        r["parity"] = {"vs": "the COO result (GCXS result converted to COO)",
+                       "bit_exact": bool(TP.same_bits(gc.data, sp.tttp(X, U).data))}
+        del gc
+    out[name] = r
+    del X, G, U
+    torch.cuda.empty_cache()
+
+    # order 2 at C4's shape: tttp against sddmm on the same inputs, alternating
+    M = N = 1_000_000
+    K = 256
+    S = _no_zero_values(rand_coo((M, N), 100_000_000, 84, torch.float32))
+    g = torch.Generator(device=DEV).manual_seed(85)
+    A, Bt = (torch.rand((n, K), generator=g, device=DEV, dtype=torch.float32) for n in (M, N))
+    t_fns = {"tttp": lambda: sp.tttp(S, [A, Bt]), "sddmm": lambda: sp.sddmm(S, A, Bt, b_transposed=True)}
+    times = {k: [] for k in t_fns}
+    for k, fn in t_fns.items():
+        fn()
+    for _ in range(5):
+        for k, fn in t_fns.items():
+            times[k].append(timeit(fn, reps=1, warm=0)[0])
+    a, b = sp.tttp(S, [A, Bt]), sp.sddmm(S, A, Bt, b_transposed=True)
+    models = _tttp_models(S, K)
+    name = "tttp order-2 C4 shape (1e6^2, nnz 1e8) R=K=256 f32 vs sddmm"
+    r = {"ms_median": round(float(np.median(times["tttp"])), 4), "ms_best": round(min(times["tttp"]), 4),
+         "sddmm_ms_median": round(float(np.median(times["sddmm"])), 4), "sddmm_ms_best": round(min(times["sddmm"]), 4),
+         "card": card, **models,
+         "values_close_to_sddmm": bool(a.nnz == b.nnz and torch.allclose(a._data_dev(), b._data_dev(), rtol=2e-5))}
+    if parity:
+        r["parity"] = _tttp_parity(S, [A, Bt], a, 10_000, 86)
+    print(name, r, flush=True)
+    out[name] = r
+    del S, A, Bt, a, b
+    torch.cuda.empty_cache()
+
+    # K9's config: tttp against the unfused expression
+    Bk = _no_zero_values(rand_coo((10_000, 10_000, 1_000), 10_000_000, 31, torch.float32))
+    g = torch.Generator(device=DEV).manual_seed(87)
+    U = [torch.rand((s, R), generator=g, device=DEV, dtype=torch.float32) + 0.05 for s in Bk.shape]
+    models = _tttp_models(Bk, R)
+    name = "tttp K9 config (1e4 x 1e4 x 1e3, nnz 1e7) R=32 f32"
+    torch.cuda.synchronize()
+    torch.cuda.reset_peak_memory_stats(DEV)
+    base = torch.cuda.memory_allocated(DEV)
+    r = rec(name, lambda: sp.tttp(Bk, U), Bk.nnz, "Gnnz_s", models["bytes"]["total"])
+    r.update({"card": card, "peak_extra_bytes": int(torch.cuda.max_memory_allocated(DEV) - base), **models})
+    got = sp.tttp(Bk, U)
+    if parity:
+        r["parity"] = _tttp_parity(Bk, U, got, 10_000, 88)
+    Uh = [u.cpu().numpy() for u in U]
+    torch.cuda.synchronize()
+    torch.cuda.reset_peak_memory_stats(DEV)
+    base = torch.cuda.memory_allocated(DEV)
+    unf = {"expression": 'einsum("ijk,ir,jr,kr->ijk", X, U0, U1, U2)', "card": _card()}
+    try:
+        ref = sp.einsum("ijk,ir,jr,kr->ijk", Bk, *Uh)
+        best, med = timeit(lambda: sp.einsum("ijk,ir,jr,kr->ijk", Bk, *Uh), reps=3, warm=1)
+        ref = ref.asformat("coo")
+        unf.update({"ms_best": round(best, 4), "ms_median": round(med, 4), "fits": True,
+                    "peak_extra_bytes": int(torch.cuda.max_memory_allocated(DEV) - base),
+                    "values_close_to_fused": bool(ref.nnz == got.nnz and np.array_equal(ref.coords, got.coords)
+                                                  and np.allclose(ref.data, got.data, rtol=2e-5, atol=0))})
+        r["speedup_vs_unfused"] = round(med / r["ms_median"], 2)
+        del ref
+    except (torch.OutOfMemoryError, RuntimeError) as e:  # the broadcast products do not fit on the card
+        unf.update({"fits": False, "error": str(e).splitlines()[0][:200],
+                    "peak_extra_bytes_before_failure": int(torch.cuda.max_memory_allocated(DEV) - base)})
+    r["unfused"] = unf
+    out[name] = r
+    del Bk, U, got
     torch.cuda.empty_cache()
     return out
 
