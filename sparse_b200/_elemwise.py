@@ -229,6 +229,29 @@ def _out_format(sparse_args):
     return COO, {}
 
 
+def _refuse_negative_exponent(exponent, T):
+    """Integer np.power raises on a negative exponent anywhere in its operands; the kernel has no error path, so the
+    exponent (scalar on the host; stored entries, fill value or dense operand with one device pass) is checked first."""
+    msg = "Integers to negative integer powers are not allowed."
+    if isinstance(exponent, COO):
+        if exponent.fill_value < 0:
+            raise ValueError(msg)
+        data = exponent._data_dev()
+    elif isinstance(exponent, np.ndarray) and exponent.ndim > 0:
+        data = D.upload(np.ascontiguousarray(exponent).reshape(-1))
+    elif D.is_device_tensor(exponent):
+        data = exponent.reshape(-1)
+    else:
+        if exponent < 0:
+            raise ValueError(msg)
+        return
+    if data.shape[0] == 0:
+        return
+    _, negative = Kn.ew_map(_BINARY[np.less], 0, Kn.cast(data, T), T.type(0), False, np.bool_)
+    if Kn.scan_flags(negative)[1]:
+        raise ValueError(msg)
+
+
 def _fill_of(func, *fills):
     """func(fill values) the way the reference evaluates it (_umath.py:516-527): NumPy values go through the ARRAY
     loop as 1-element arrays, Python scalars stay weak scalars.  NumPy's scalar and array loops are not bit-identical
@@ -530,6 +553,8 @@ class _Elemwise:
         if T in _WIDE_FOR and func not in _NOT_VIA_WIDE:
             return self._via_wide(func, T, out_dt)
         _check_compute_dtype(T, func)
+        if func is np.power and T.kind == "i":
+            _refuse_negative_exponent(b, T)
         if op < 32 and out_dt == np.bool_:
             raise TypeError(f"sparse_b200: {func.__name__} with boolean output is outside the CUDA dtype matrix")
         shape = self.shape

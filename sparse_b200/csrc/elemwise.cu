@@ -12,6 +12,7 @@
 // Also here: COO (x) scalar / unary maps and COO (x) dense-ndarray gathers (mask (True, None), _umath.py:606-608),
 // and the broadcast expansion kernel for non-trailing broadcast axes (_get_expanded_coords_data, :220-277).
 #include <cub/cub.cuh>
+#include <limits>
 #include <type_traits>
 
 #include "common.cuh"
@@ -69,6 +70,19 @@ __device__ __forceinline__ T raw_or(T a, T b) {
     }
 }
 
+// Integer power by squaring with wrapping products: multiplication modulo 2^bits is associative, so this equals
+// NumPy's loop bit for bit (0 ** 0 = 1).  b >= 0: the host refuses negative exponents.  Not inlined: a copy of the loop
+// in each of the merge kernel's 7 unrolled items would add register spills to every integer instantiation.
+template <typename T>
+__device__ __noinline__ T int_pow(T a, T b) {
+    T r = T(1), base = a;
+    for (auto e = (typename std::make_unsigned<T>::type)b; e != 0; e >>= 1) {
+        if (e & 1) r = mul_rn(r, base);
+        base = mul_rn(base, base);
+    }
+    return r;
+}
+
 template <typename T>
 __device__ __forceinline__ T bin_apply(int op, T a, T b) {
     if (op >= OP_SEL_X && op <= OP_BITOR_RAW) {
@@ -85,8 +99,9 @@ __device__ __forceinline__ T bin_apply(int op, T a, T b) {
             // NaN propagates; ties (+0 vs -0) return the SECOND operand, like NumPy's x86 SIMD loops (maxpd/minpd)
             case OP_MAXIMUM: return (is_nan(a) || is_nan(b)) ? (is_nan(a) ? a : b) : (a > b ? a : b);
             case OP_MINIMUM: return (is_nan(a) || is_nan(b)) ? (is_nan(a) ? a : b) : (a < b ? a : b);
-            case OP_FMAX: return is_nan(a) ? b : (is_nan(b) ? a : (a > b ? a : b));
-            case OP_FMIN: return is_nan(a) ? b : (is_nan(b) ? a : (a < b ? a : b));
+            // a NaN operand loses; of two NaNs the FIRST is returned, bits kept (NumPy: a >= b || isnan(b) ? a : b)
+            case OP_FMAX: return is_nan(b) ? a : (is_nan(a) ? b : (a > b ? a : b));
+            case OP_FMIN: return is_nan(b) ? a : (is_nan(a) ? b : (a < b ? a : b));
             case OP_NANREPLACE: return is_nan(a) ? b : a;
             case OP_POW: return pow(a, b);
             case OP_FLOORDIV: {
@@ -118,6 +133,7 @@ __device__ __forceinline__ T bin_apply(int op, T a, T b) {
             case OP_ADD: return add_rn(a, b);
             case OP_SUB: return (T)((typename std::make_unsigned<T>::type)a - (typename std::make_unsigned<T>::type)b);
             case OP_MUL: return mul_rn(a, b);
+            case OP_POW: return int_pow(a, b);
             case OP_MAXIMUM: case OP_FMAX: return a >= b ? a : b;
             case OP_MINIMUM: case OP_FMIN: return a <= b ? a : b;
             case OP_FLOORDIV: {
@@ -198,8 +214,10 @@ __device__ __forceinline__ T un_apply(int op, T a) {
             case U_RINT: return rint(a);
             case U_RECIP: return T(1) / a;
             case U_CBRT: return cbrt(a);
-            case U_DEG2RAD: return a * T(0.017453292519943295);
-            case U_RAD2DEG: return a * T(57.29577951308232);
+            // NumPy's constants: pi / 180 and 180 / pi rounded in T (180 / pi in float is 57.295776f, not the float
+            // nearest to 180 / pi in double, 57.29578f)
+            case U_DEG2RAD: { constexpr T k = T(3.14159265358979323846) / T(180); return a * k; }
+            case U_RAD2DEG: { constexpr T k = T(180) / T(3.14159265358979323846); return a * k; }
             default: return T(0);
         }
     } else {
@@ -210,6 +228,9 @@ __device__ __forceinline__ T un_apply(int op, T a) {
             case U_SQUARE: return mul_rn(a, a);
             case U_SIGN: return a > 0 ? T(1) : (a < 0 ? T(-1) : T(0));
             case U_INVERT: return ~a;
+            case U_FLOOR: case U_CEIL: case U_TRUNC: return a;  // NumPy >= 2 keeps the integer dtype: the identity
+            // NumPy computes (T)(1.0 / a): 1 -> 1, -1 -> -1, 0 -> (T)inf, which is the minimum on x86-64, else 0
+            case U_RECIP: return (a == T(1) || a == T(-1)) ? a : (a == T(0) ? std::numeric_limits<T>::min() : T(0));
             default: return T(0);
         }
     }
