@@ -107,13 +107,18 @@ def mttkrp(B, Dm, Cm):
 _FORCE_WIDE_INDEX = False
 
 
+def _index_limit(X):
+    """The largest value X's coordinate arrays must hold: int32 suffices below 2**31 - 1."""
+    return 2**63 if _FORCE_WIDE_INDEX else max(*X.shape, X.nnz)
+
+
 def _mode_stream(X, mode):
     """Coordinate rows (a list of N device index tensors) and values of X's entries in the order of the mode stream
     S_mode: C order for mode 0, C order sorted stably by coordinate `mode` otherwise.  Cached on X per mode."""
     from ._gcxs import GCXS
     from ._utils import key_bits
 
-    limit = 2**63 if _FORCE_WIDE_INDEX else max(*X.shape, X.nnz)
+    limit = _index_limit(X)
     key = (mode, limit < 2**31 - 1)
     cache = X._mode_streams
     if cache is not None and key in cache:
@@ -132,9 +137,11 @@ def _mode_stream(X, mode):
     return stream
 
 
-def _tensor_and_factors(name, X, factors, mode):
+def _tensor_and_factors(name, X, factors, mode, one_rank):
     """Checks shared by mttkrp_mode, ttmc_mode and tttp: (order N, mode in 0..N-1, the factors as a list with the other
-    modes' ones as NumPy arrays or device tensors, the other modes ascending).  `mode` None (tttp) reads every factor."""
+    modes' ones as NumPy arrays or device tensors, the other modes ascending, the result dtype T, the ranks: a list of N
+    with ranks[m] = factors[m].shape[1] for the other modes and 0 for `mode`).  `mode` None (tttp) reads every factor.
+    With `one_rank` every factor read must have the same number of columns."""
     from ._gcxs import GCXS
 
     if not isinstance(X, (COO, GCXS)):
@@ -152,10 +159,38 @@ def _tensor_and_factors(name, X, factors, mode):
     if len(factors) != N:
         raise ValueError(f"{name}: {len(factors)} factors for an order-{N} tensor")
     others = [m for m in range(N) if m != mode]
+    if mode is None:
+        for m in others:
+            if factors[m] is None:
+                raise ValueError(f"{name}: factor {m} is None ({name} reads every factor)")
     for m in others:
         if not D.is_device_tensor(factors[m]):
             factors[m] = np.asarray(factors[m])
-    return N, mode, factors, others
+    ranks = [0] * N
+    R = int(factors[others[0]].shape[1]) if factors[others[0]].ndim == 2 else -1
+    for m in others:
+        f = factors[m]
+        if f.ndim != 2 or int(f.shape[0]) != X.shape[m] or (one_rank and int(f.shape[1]) != R):
+            expected = f"({X.shape[m]}, R) with one R for all factors" if one_rank else f"({X.shape[m]}, R_{m})"
+            raise ValueError(f"{name}: shape mismatch X{X.shape}, factor {m} {tuple(f.shape)} (expected {expected})")
+        ranks[m] = int(f.shape[1])
+    T = np.result_type(X.dtype, *(_dense_dt(factors[m]) for m in others))
+    if T not in (np.dtype("float32"), np.dtype("float64")):
+        raise TypeError(f"{name}: dtype {T} is outside the CUDA dtype matrix (float32, float64)")
+    return N, mode, factors, T, ranks
+
+
+def _mode_product(X, factors, mode, T, W, kernel, rank_arg):
+    """The dense (X.shape[mode], W) result of mttkrp_mode / ttmc_mode after their checks: zeros when nothing is
+    stored, else `kernel` (Kn.mttkrp_mode or Kn.ttmc_mode, given `rank_arg`) over the cached mode stream."""
+    N, rows = X.ndim, X.shape[mode]
+    if X.nnz == 0 or rows == 0 or W == 0:
+        out = Kn.full(rows * W, 0, T).reshape(rows, W)
+    else:
+        coords, vals = _mode_stream(X, mode)
+        fac = [None if m == mode else _dense_dev(factors[m], T) for m in range(N)]
+        out = kernel(coords, Kn.cast(vals, T), fac, mode, rows, rank_arg)
+    return _return_dense(out, [f for f in factors if f is not None])
 
 
 def mttkrp_mode(X, factors, mode):
@@ -177,24 +212,9 @@ def mttkrp_mode(X, factors, mode):
     dropped when X's contents are replaced, and are not copied or pickled).  A cached mode holds
     (N * index bytes + value bytes) * nnz of device memory -- index bytes 4 when every extent and nnz fit int32, else 8.
     """
-    N, mode, factors, others = _tensor_and_factors("mttkrp_mode", X, factors, mode)
-    R = int(factors[others[0]].shape[1]) if factors[others[0]].ndim == 2 else -1
-    for m in others:
-        f = factors[m]
-        if f.ndim != 2 or int(f.shape[0]) != X.shape[m] or int(f.shape[1]) != R:
-            raise ValueError(f"mttkrp_mode: shape mismatch X{X.shape}, factor {m} {tuple(f.shape)} "
-                             f"(expected ({X.shape[m]}, R) with one R for all factors)")
-    T = np.result_type(X.dtype, *(_dense_dt(factors[m]) for m in others))
-    if T not in (np.dtype("float32"), np.dtype("float64")):
-        raise TypeError(f"mttkrp_mode: dtype {T} is outside the CUDA dtype matrix (float32, float64)")
-    rows = X.shape[mode]
-    if X.nnz == 0 or rows == 0 or R == 0:
-        out = Kn.full(rows * R, 0, T).reshape(rows, R)
-    else:
-        coords, vals = _mode_stream(X, mode)
-        fac = [None if m == mode else _dense_dev(factors[m], T) for m in range(N)]
-        out = Kn.mttkrp_mode(coords, Kn.cast(vals, T), fac, mode, rows, R)
-    return _return_dense(out, [f for f in factors if f is not None])
+    N, mode, factors, T, ranks = _tensor_and_factors("mttkrp_mode", X, factors, mode, True)
+    R = max(ranks)  # the one R of the other factors (ranks[mode] is 0)
+    return _mode_product(X, factors, mode, T, R, Kn.mttkrp_mode, R)
 
 
 def ttmc_mode(X, factors, mode):
@@ -222,29 +242,12 @@ def ttmc_mode(X, factors, mode):
     ((N * index bytes + value bytes) * nnz, as described there); and, during the call, a scratch array of
     2 * ceil(nnz / 512) * W' * itemsize bytes (W' = W rounded up to a multiple of 4) for the rows that cross chunks.
     """
-    N, mode, factors, others = _tensor_and_factors("ttmc_mode", X, factors, mode)
-    ranks = [0] * N
-    for m in others:
-        f = factors[m]
-        if f.ndim != 2 or int(f.shape[0]) != X.shape[m]:
-            raise ValueError(f"ttmc_mode: shape mismatch X{X.shape}, factor {m} {tuple(f.shape)} "
-                             f"(expected ({X.shape[m]}, R_{m}))")
-        ranks[m] = int(f.shape[1])
-    T = np.result_type(X.dtype, *(_dense_dt(factors[m]) for m in others))
-    if T not in (np.dtype("float32"), np.dtype("float64")):
-        raise TypeError(f"ttmc_mode: dtype {T} is outside the CUDA dtype matrix (float32, float64)")
-    W = int(np.prod([ranks[m] for m in others], dtype=object))
+    N, mode, factors, T, ranks = _tensor_and_factors("ttmc_mode", X, factors, mode, False)
+    W = int(np.prod([ranks[m] for m in range(N) if m != mode], dtype=object))
     if W > Kn.ttmc_mode_max_width():
         raise ValueError(f"ttmc_mode: {W} output columns (the product of the other modes' ranks) exceed the limit of "
                          f"{Kn.ttmc_mode_max_width()}")
-    rows = X.shape[mode]
-    if X.nnz == 0 or rows == 0 or W == 0:
-        out = Kn.full(rows * W, 0, T).reshape(rows, W)
-    else:
-        coords, vals = _mode_stream(X, mode)
-        fac = [None if m == mode else _dense_dev(factors[m], T) for m in range(N)]
-        out = Kn.ttmc_mode(coords, Kn.cast(vals, T), fac, mode, rows, ranks)
-    return _return_dense(out, [f for f in factors if f is not None])
+    return _mode_product(X, factors, mode, T, W, Kn.ttmc_mode, ranks)
 
 
 def _gcxs_coords(X, limit):
@@ -290,26 +293,14 @@ def tttp(X, factors):
     """
     from ._gcxs import GCXS
 
-    given = list(factors)
-    N, _, factors, _ = _tensor_and_factors("tttp", X, given, None)
-    for m in range(N):
-        if given[m] is None:
-            raise ValueError(f"tttp: factor {m} is None (tttp reads every factor)")
-    R = int(factors[0].shape[1]) if factors[0].ndim == 2 else -1
-    for m, f in enumerate(factors):
-        if f.ndim != 2 or int(f.shape[0]) != X.shape[m] or int(f.shape[1]) != R:
-            raise ValueError(f"tttp: shape mismatch X{X.shape}, factor {m} {tuple(f.shape)} "
-                             f"(expected ({X.shape[m]}, R) with one R for all factors)")
-    T = np.result_type(X.dtype, *(_dense_dt(f) for f in factors))
-    if T not in (np.dtype("float32"), np.dtype("float64")):
-        raise TypeError(f"tttp: dtype {T} is outside the CUDA dtype matrix (float32, float64)")
-    limit = 2**63 if _FORCE_WIDE_INDEX else max(*X.shape, X.nnz)
+    _, _, factors, T, ranks = _tensor_and_factors("tttp", X, factors, None, True)
+    R = ranks[0]
     if isinstance(X, GCXS):
         data, indices, indptr = X._dev()
         if X.nnz == 0:
             out = Kn.full(0, 0, T)
         else:
-            out = Kn.tttp(_gcxs_coords(X, limit), Kn.cast(data, T), [_dense_dev(f, T) for f in factors], R)
+            out = Kn.tttp(_gcxs_coords(X, _index_limit(X)), Kn.cast(data, T), [_dense_dev(f, T) for f in factors], R)
         res = GCXS._from_device(out, indices, indptr, X.shape, X.compressed_axes, T.type(0))
         res._idx_vis = X._idx_vis
         res._prune()  # drops results that are bitwise +0, as X * model does

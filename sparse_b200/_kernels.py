@@ -656,32 +656,38 @@ def mttkrp_mode_chunk() -> int:
     return int(_lib.load().b2s_mttkrp_mode_chunk())
 
 
-def mttkrp_mode(coords, vals, factors, mode, rows, R):
-    """out[i, r] = sum over the stream entries e with coords[mode][e] = i of vals[e] * prod_{m != mode}
-    factors[m][coords[m][e], r], in the fixed order of b2s_mttkrp_mode.  `coords` (N index tensors, one width) and
-    `vals` are the mode stream; factors[mode] is not read."""
-    t = _t()
-    N = len(coords)
-    dt = D.np_dtype(vals)
+def _factor_args(coords, vals, factors, ranks, skip=None):
+    """The pointer arrays of the sparse-tensor entry points: coordinate pointers, factor pointers, their row strides
+    (factor m has ranks[m] columns), and the factors passed (contiguous copies where needed, kept alive by the caller
+    until the launch is enqueued: the caching allocator orders their reuse).  Factor `skip` is not read."""
     assert all(c.dtype == coords[0].dtype for c in coords)
     fac, ld, keep = [], [], []
     for m, f in enumerate(factors):
-        if m == mode:
+        R = int(ranks[m])
+        if m == skip:
             fac.append(0)
             ld.append(R)
             continue
         assert f.dtype == vals.dtype
         if R > 1 and f.stride(1) != 1:
             f = f.contiguous()
-        keep.append(f)  # a contiguous copy lives until the launch is enqueued (the caching allocator orders its reuse)
+        keep.append(f)
         fac.append(D.ptr(f))
         ld.append(f.stride(0) if f.shape[0] > 1 else R)
-    out = t.empty((rows, R), dtype=vals.dtype, device=vals.device)
-    ptrs = (ctypes.c_void_p * N)(*[D.ptr(c) for c in coords])
-    fptrs = (ctypes.c_void_p * N)(*fac)
-    rc = _lib.load().b2s_mttkrp_mode(i32(D.dtype_code(dt)), i32(_idx_bytes(coords[0])), i32(N), i32(mode),
-                                     i64(vals.shape[0]), i64(rows), i64(R), ptrs, vp(D.ptr(vals)), fptrs, _i64arr(ld),
-                                     vp(D.ptr(out)), i64(R), _sp())
+    N = len(coords)
+    return (ctypes.c_void_p * N)(*[D.ptr(c) for c in coords]), (ctypes.c_void_p * N)(*fac), _i64arr(ld), keep
+
+
+def mttkrp_mode(coords, vals, factors, mode, rows, R):
+    """out[i, r] = sum over the stream entries e with coords[mode][e] = i of vals[e] * prod_{m != mode}
+    factors[m][coords[m][e], r], in the fixed order of b2s_mttkrp_mode.  `coords` (N index tensors, one width) and
+    `vals` are the mode stream; factors[mode] is not read."""
+    N = len(coords)
+    ptrs, fptrs, ld, keep = _factor_args(coords, vals, factors, [R] * N, mode)
+    out = _t().empty((rows, R), dtype=vals.dtype, device=vals.device)
+    rc = _lib.load().b2s_mttkrp_mode(i32(D.dtype_code(D.np_dtype(vals))), i32(_idx_bytes(coords[0])), i32(N),
+                                     i32(mode), i64(vals.shape[0]), i64(rows), i64(R), ptrs, vp(D.ptr(vals)), fptrs,
+                                     ld, vp(D.ptr(out)), i64(R), _sp())
     _lib.check(rc, "b2s_mttkrp_mode")
     return out
 
@@ -699,33 +705,16 @@ def ttmc_mode(coords, vals, factors, mode, rows, ranks):
     factors[m][coords[m][e], r_m], col the C-order index of (r_m for m != mode), in the fixed order of b2s_ttmc_mode.
     `coords` (N index tensors, one width) and `vals` are the mode stream; `ranks[m]` is factors[m].shape[1];
     factors[mode] is not read."""
-    t = _t()
     N = len(coords)
-    dt = D.np_dtype(vals)
-    assert all(c.dtype == coords[0].dtype for c in coords)
     W = 1
     for m in range(N):
         if m != mode:
             W *= int(ranks[m])
-    fac, ld, keep = [], [], []
-    for m, f in enumerate(factors):
-        if m == mode:
-            fac.append(0)
-            ld.append(0)
-            continue
-        assert f.dtype == vals.dtype
-        R = int(ranks[m])
-        if R > 1 and f.stride(1) != 1:
-            f = f.contiguous()
-        keep.append(f)  # a contiguous copy lives until the launch is enqueued (the caching allocator orders its reuse)
-        fac.append(D.ptr(f))
-        ld.append(f.stride(0) if f.shape[0] > 1 else R)
-    out = t.empty((rows, W), dtype=vals.dtype, device=vals.device)
-    ptrs = (ctypes.c_void_p * N)(*[D.ptr(c) for c in coords])
-    fptrs = (ctypes.c_void_p * N)(*fac)
-    rc = _lib.load().b2s_ttmc_mode(i32(D.dtype_code(dt)), i32(_idx_bytes(coords[0])), i32(N), i32(mode),
-                                   i64(vals.shape[0]), i64(rows), _i64arr([int(r) for r in ranks]), ptrs,
-                                   vp(D.ptr(vals)), fptrs, _i64arr(ld), vp(D.ptr(out)), i64(W), _sp())
+    ptrs, fptrs, ld, keep = _factor_args(coords, vals, factors, ranks, mode)
+    out = _t().empty((rows, W), dtype=vals.dtype, device=vals.device)
+    rc = _lib.load().b2s_ttmc_mode(i32(D.dtype_code(D.np_dtype(vals))), i32(_idx_bytes(coords[0])), i32(N),
+                                   i32(mode), i64(vals.shape[0]), i64(rows), _i64arr([int(r) for r in ranks]), ptrs,
+                                   vp(D.ptr(vals)), fptrs, ld, vp(D.ptr(out)), i64(W), _sp())
     _lib.check(rc, "b2s_ttmc_mode")
     return out
 
@@ -736,23 +725,11 @@ def ttmc_mode(coords, vals, factors, mode, rows, ranks):
 def tttp(coords, vals, factors, R):
     """out[e] = vals[e] * sum_r prod_m factors[m][coords[m][e], r], in the fixed order of b2s_tttp.  `coords` (N index
     tensors, one width) and `vals` give the entries in the order of the result; every factor is read."""
-    t = _t()
     N = len(coords)
-    dt = D.np_dtype(vals)
-    assert all(c.dtype == coords[0].dtype for c in coords)
-    fac, ld, keep = [], [], []
-    for f in factors:
-        assert f.dtype == vals.dtype
-        if R > 1 and f.stride(1) != 1:
-            f = f.contiguous()
-        keep.append(f)  # a contiguous copy lives until the launch is enqueued (the caching allocator orders its reuse)
-        fac.append(D.ptr(f))
-        ld.append(f.stride(0) if f.shape[0] > 1 else R)
-    out = t.empty_like(vals)
-    ptrs = (ctypes.c_void_p * N)(*[D.ptr(c) for c in coords])
-    fptrs = (ctypes.c_void_p * N)(*fac)
-    rc = _lib.load().b2s_tttp(i32(D.dtype_code(dt)), i32(_idx_bytes(coords[0])), i32(N), i64(vals.shape[0]), i64(R),
-                              ptrs, vp(D.ptr(vals)), fptrs, _i64arr(ld), vp(D.ptr(out)), _sp())
+    ptrs, fptrs, ld, keep = _factor_args(coords, vals, factors, [R] * N)
+    out = _t().empty_like(vals)
+    rc = _lib.load().b2s_tttp(i32(D.dtype_code(D.np_dtype(vals))), i32(_idx_bytes(coords[0])), i32(N),
+                              i64(vals.shape[0]), i64(R), ptrs, vp(D.ptr(vals)), fptrs, ld, vp(D.ptr(out)), _sp())
     _lib.check(rc, "b2s_tttp")
     return out
 

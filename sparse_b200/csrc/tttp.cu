@@ -11,7 +11,7 @@
 // carries across r-tiles.  The products q_r are independent; only that sum is serial, so the result is the order of
 // include/sparse_b200.h whatever the grid, and the vector (VEC = 16 B / itemsize) and scalar (VEC = 1) forms are
 // bit-identical.  No atomics, no scratch memory.
-#include "common.cuh"
+#include "tensor_modes.cuh"
 
 namespace b2s {
 
@@ -22,29 +22,7 @@ constexpr int kSteps = 32 / kEntriesPerStep;          // gather steps per block 
 constexpr int kWarps = 8;                            // warps per CTA
 
 template <typename I>
-struct TttpModes {
-    const I *coord[kMaxOrder];
-    const void *fac[kMaxOrder];
-    int64_t ld[kMaxOrder];
-};
-
-template <typename T, int VEC>
-struct alignas(sizeof(T) * VEC) TPack {
-    T v[VEC];
-};
-
-template <typename T, int VEC>
-__device__ __forceinline__ TPack<T, VEC> t_load(const T *p, uint64_t pol) {
-    TPack<T, VEC> r;
-    if constexpr (sizeof(T) * VEC == 16) {
-        const uint4 u = ldg_nc_v4_hint(p, pol);
-        memcpy(&r, &u, 16);
-    } else {
-        static_assert(VEC == 1, "only 16-byte or scalar packs");
-        r.v[0] = __ldg(p);
-    }
-    return r;
-}
+using TttpModes = ModeArrays<I, kMaxOrder>;
 
 template <typename T, typename I, int VEC>
 __global__ void __launch_bounds__(kWarps * 32)
@@ -75,19 +53,19 @@ tttp_kernel(const TttpModes<I> md, const int order, const T *__restrict__ vals, 
     for (int64_t r0 = 0; r0 < R; r0 += RT) {
         const int64_t col = r0 + (int64_t)sub * VEC;
         const bool col_ok = col < R;  // VEC divides R on the vector path: a pack is all in or all out
-        TPack<T, VEC> p[kSteps];
+        MPack<T, VEC> p[kSteps];
         // q = ((U_0 * U_1) * U_2) * ... over the modes in ascending order, each product rounded
 #pragma unroll
         for (int m = 0; m < kMaxOrder; ++m) {
             if (m < order) {
                 const T *fm = (const T *)md.fac[m] + col;
                 const int64_t ldm = md.ld[m];
-                TPack<T, VEC> f[kSteps];
+                MPack<T, VEC> f[kSteps];
 #pragma unroll
                 for (int s = 0; s < kSteps; ++s) {
                     const int e = s * kEntriesPerStep + grp;
                     const I ix = __shfl_sync(FULL, c[m], e);
-                    if (e < cnt && col_ok) f[s] = t_load<T, VEC>(fm + (int64_t)ix * ldm, pol);
+                    if (e < cnt && col_ok) f[s] = m_load<T, VEC>(fm + (int64_t)ix * ldm, pol);
                     else {
 #pragma unroll
                         for (int k = 0; k < VEC; ++k) f[s].v[k] = T(0);
@@ -156,26 +134,19 @@ extern "C" {
 int b2s_tttp(int dtype, int idx_bytes, int order, int64_t nnz, int64_t R, const void *const *coords_host,
              const void *vals_dev, const void *const *factors_host, const int64_t *ld_host, void *out_vals_dev,
              void *stream) {
-    B2S_REQUIRE(dtype == B2S_F32 || dtype == B2S_F64, B2S_ERR_UNSUPPORTED, "tttp: dtype %d (f32/f64 only)", dtype);
-    B2S_REQUIRE(idx_bytes == 4 || idx_bytes == 8, B2S_ERR_INVALID, "tttp: idx_bytes");
-    B2S_REQUIRE(order >= 2 && order <= 8, B2S_ERR_INVALID, "tttp: order %d outside 2..8", order);
-    B2S_REQUIRE(nnz >= 0 && R >= 0, B2S_ERR_INVALID, "tttp: negative size");
-    B2S_REQUIRE(nnz / 256 < INT32_MAX, B2S_ERR_INVALID, "tttp: nnz %lld exceeds one grid", (long long)nnz);
+    const char *op = "tttp";
+    int rc = check_tensor(op, dtype, idx_bytes, order);
+    if (rc) return rc;
+    B2S_REQUIRE(nnz >= 0 && R >= 0, B2S_ERR_INVALID, "%s: negative size", op);
+    B2S_REQUIRE(nnz / 256 < INT32_MAX, B2S_ERR_INVALID, "%s: nnz %lld exceeds one grid", op, (long long)nnz);
     if (nnz == 0) return B2S_OK;
-    B2S_REQUIRE(coords_host != nullptr && factors_host != nullptr && ld_host != nullptr, B2S_ERR_INVALID,
-                "tttp: NULL pointer array");
-    for (int m = 0; m < order; ++m)
-        B2S_REQUIRE(ld_host[m] >= R, B2S_ERR_INVALID, "tttp: ld of factor %d < R", m);
+    rc = check_factors(op, order, -1, coords_host, factors_host, ld_host, R, nullptr);
+    if (rc) return rc;
     cudaStream_t s = (cudaStream_t)stream;
-#define B2S_TT(T, I) \
-    return tttp_impl<T, I>(order, nnz, R, coords_host, vals_dev, factors_host, ld_host, out_vals_dev, s)
-    if (dtype == B2S_F32) {
-        if (idx_bytes == 4) B2S_TT(float, int32_t);
-        B2S_TT(float, int64_t);
-    }
-    if (idx_bytes == 4) B2S_TT(double, int32_t);
-    B2S_TT(double, int64_t);
-#undef B2S_TT
+    return dispatch_tensor(dtype, idx_bytes, [&](auto t, auto i) {
+        return tttp_impl<decltype(t), decltype(i)>(order, nnz, R, coords_host, vals_dev, factors_host, ld_host,
+                                                   out_vals_dev, s);
+    });
 }
 
 }  // extern "C"

@@ -24,6 +24,24 @@ def _ordered_sums(x, starts, lens):
     return acc
 
 
+def _chunked_row_sums(p, row, rows):
+    """(rows, ...) result of the products p (one per stream entry, rows of index `row`): partials per (chunk, row) run
+    in stream order, row results over the chunks in chunk order, every sum starting from +0, rows without entries +0."""
+    out = np.zeros((rows,) + p.shape[1:], dtype=p.dtype)
+    ch = Kn.mttkrp_mode_chunk()  # the library's constant (needs no device)
+    pos = np.arange(len(row))
+    head = np.ones(len(row), dtype=bool)
+    head[1:] = (row[1:] != row[:-1]) | (pos[1:] % ch == 0)
+    starts = np.flatnonzero(head)
+    partial = _ordered_sums(p, starts, np.diff(np.append(starts, len(row))))
+    prow = row[starts]
+    rhead = np.ones(len(starts), dtype=bool)
+    rhead[1:] = prow[1:] != prow[:-1]
+    rstarts = np.flatnonzero(rhead)
+    out[prow[rstarts]] = _ordered_sums(partial, rstarts, np.diff(np.append(rstarts, len(starts))))
+    return out
+
+
 def mttkrp_mode(coords, vals, factors, mode, rows, R):
     """Products in ascending mode order, partials per (chunk, row) run in stream order, row results over the chunks
     in chunk order, every sum starting from +0.  Same argument contract as the real wrapper."""
@@ -40,16 +58,5 @@ def mttkrp_mode(coords, vals, factors, mode, rows, R):
             for m in range(len(c)):
                 if m != mode:
                     p = p * factors[m].detach().numpy()[c[m]]
-        ch = Kn.mttkrp_mode_chunk()  # the library's constant (needs no device)
-        row = c[mode]
-        pos = np.arange(len(v))
-        head = np.ones(len(v), dtype=bool)
-        head[1:] = (row[1:] != row[:-1]) | (pos[1:] % ch == 0)
-        starts = np.flatnonzero(head)
-        partial = _ordered_sums(p, starts, np.diff(np.append(starts, len(v))))
-        prow = row[starts]
-        rhead = np.ones(len(starts), dtype=bool)
-        rhead[1:] = prow[1:] != prow[:-1]
-        rstarts = np.flatnonzero(rhead)
-        out[prow[rstarts]] = _ordered_sums(partial, rstarts, np.diff(np.append(rstarts, len(starts))))
+        out = _chunked_row_sums(p, c[mode], rows)
     return torch.from_numpy(out)

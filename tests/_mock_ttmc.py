@@ -10,9 +10,8 @@ from __future__ import annotations
 import numpy as np
 import torch
 
-from _mock_mttkrp import _ordered_sums
+from _mock_mttkrp import _chunked_row_sums
 from sparse_b200 import _device as D
-from sparse_b200 import _kernels as Kn
 
 
 def ttmc_mode(coords, vals, factors, mode, rows, ranks):
@@ -26,7 +25,7 @@ def ttmc_mode(coords, vals, factors, mode, rows, ranks):
     for m in range(len(coords)):
         if m != mode:
             W *= int(ranks[m])
-    c =[x.detach().numpy().astype(np.int64) for x in coords]
+    c = [x.detach().numpy().astype(np.int64) for x in coords]
     v = vals.detach().numpy()
     out = np.zeros((rows, W), dtype=v.dtype)
     if len(v) and rows and W:
@@ -36,16 +35,5 @@ def ttmc_mode(coords, vals, factors, mode, rows, ranks):
                 if m != mode:
                     f = factors[m].detach().numpy()[c[m]]
                     p = (p[:, :, None] * f[:, None, :]).reshape(len(v), -1)
-        ch = Kn.mttkrp_mode_chunk()  # the library's constant (needs no device)
-        row = c[mode]
-        pos = np.arange(len(v))
-        head = np.ones(len(v), dtype=bool)
-        head[1:] = (row[1:] != row[:-1]) | (pos[1:] % ch == 0)
-        starts = np.flatnonzero(head)
-        partial = _ordered_sums(p, starts, np.diff(np.append(starts, len(v))))
-        prow = row[starts]
-        rhead = np.ones(len(starts), dtype=bool)
-        rhead[1:] = prow[1:] != prow[:-1]
-        rstarts = np.flatnonzero(rhead)
-        out[prow[rstarts]] = _ordered_sums(partial, rstarts, np.diff(np.append(rstarts, len(starts))))
+        out = _chunked_row_sums(p, c[mode], rows)
     return torch.from_numpy(out)
