@@ -366,6 +366,43 @@ int b2s_tttp(int dtype, int idx_bytes, int order, int64_t nnz, int64_t R, const 
              const void *vals_dev, const void *const *factors_host, const int64_t *ld_host, void *out_vals_dev,
              void *stream);
 
+/* ---- mode-n tensor times matrix of a sparse tensor of order 2..8, with a sparse result (K14, ttm.cu; TTM / TTV, the
+ * reference computes it only as tensordot(X, U, axes=([n], [0]))) ------------------------------------------------------
+ * Y[i_0, ..., r, ..., i_{N-1}] = sum_{i_n} X[i_0, ..., i_n, ..., i_{N-1}] * U[i_n, r], r < R, for the n_fibers fibers of
+ * the FIBER STREAM of mode n: the entries sorted by the key over (the other modes ascending, then n), with
+ *  - kcoord_dev / vals_dev: each entry's coordinate i_n and value, in stream order (idx_bytes wide);
+ *  - fptr_dev[n_fibers + 1]: the fibers, runs of entries sharing every coordinate but i_n;
+ *  - fgroup_dev[n_fibers] / gptr_dev: each fiber's group, and the groups as runs of fibers sharing the coordinates
+ *    before n (idx_bytes wide);
+ *  - fkey_dev / pkey_dev[n_fibers]: each fiber's C-order linear coordinate over the other modes, and over the modes
+ *    before n alone (P), so that Q = fkey - P * q_ext is the one over the modes after n (q_ext: their extents' product).
+ * U_dev is (X.shape[n] x R) with row stride ldu >= R.  For every fiber f (group start g0, group size s_g) and r < R the
+ * call writes, at slot = R * g0 + r * s_g + (f - g0) of the n_fibers * R caller-allocated outputs, the value y, its key
+ * (P * R + r) * q_ext + Q (the C-order linear index in Y's shape) and the keep flag y != 0.  The slots are in key order.
+ * long_ids_dev[n_long] (int64, ascending) must list exactly the fibers with more than long_min entries: each gets whole
+ * CTAs that stage a chunk of its products in shared memory (the short-fiber lanes skip them), so skewed fiber lengths
+ * do not hold the grid.  No atomics, no scratch memory, no stream synchronisation.
+ *
+ * Fixed order of operations (results are reproducible bit for bit, whatever the grid, index width, stream, column
+ * path, long_min or fiber role):
+ *  1. A fiber is the set of stored entries that share every coordinate except i_n.
+ *  2. y(f, r) = ((+0 + v_1 * U[k_1, r]) + v_2 * U[k_2, r]) + ... over the fiber's entries in ascending k = i_n, each
+ *     product and each sum rounded separately; no FMA contraction.
+ *  3. An entry of Y is stored iff y != 0: +-0 are dropped, NaN is kept (the caller's compaction, from the flags).
+ * This is K1's order on the matricised operand (rows = the other modes in C order, columns = i_n), followed by
+ * b2s_dense_to_csr mode 0: for a canonical COO X the result equals tensordot(X, U, axes=([n], [0]), return_type=COO)
+ * with the R axis moved to position n, bit for bit.
+ */
+int b2s_ttm_mode(int dtype, int idx_bytes, int64_t n_fibers, int64_t R, int64_t q_ext, const void *kcoord_dev,
+                 const void *vals_dev, const void *fptr_dev, const void *fgroup_dev, const void *gptr_dev,
+                 const int64_t *fkey_dev, const int64_t *pkey_dev, const int64_t *long_ids_dev, int64_t n_long,
+                 int64_t long_min, const void *u_dev, int64_t ldu, void *out_vals_dev, int64_t *out_keys_dev,
+                 uint8_t *out_flags_dev, void *stream);
+/* flags_out[f] = 1 iff fiber f has more than long_min entries (fptr_dev[n_fibers + 1], idx_bytes wide).  The ascending
+ * indices of the flagged fibers are b2s_ttm_mode's long_ids (n_long of them), with the same long_min. */
+int b2s_ttm_mode_long_flags(int idx_bytes, int64_t n_fibers, const void *fptr_dev, int64_t long_min,
+                            uint8_t *flags_out_dev, void *stream);
+
 /* ---- masked sparse x sparse product (K11, masked_spgemm.cu; examples/triangles_example.py) ------------------------
  * out_vals[p] = value of mask * (A @ B) at every stored mask entry p, given the mask as CSR (m_indptr over the M rows,
  * m_cols, m_vals already in the output dtype `dtype_out`), A as CSR (M x K) and B^T as CSR (N x K, i.e. B by

@@ -144,7 +144,8 @@ class COO(SparseArray):
             self._canonicalise(check_sort=not sorted, sum_dups=has_duplicates, prune=prune)
 
     # ---- construction helpers ------------------------------------------------------------------------
-    # mode streams of mttkrp_mode ({(mode, int32 indices): (coordinate rows, values)}); belong to the current contents
+    # mode streams of mttkrp_mode ({(mode, int32 indices): (coordinate rows, values)}) and fiber streams of ttm_mode
+    # ({("fiber", mode, int32 indices): ...}); belong to the current contents
     _mode_streams = None
 
     def _copy_from(self, other):

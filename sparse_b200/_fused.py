@@ -11,6 +11,8 @@ mttkrp_mode(X, factors, mode) generalises mttkrp to any mode of a tensor of orde
 counterpart in the reference beyond the unfused broadcast expression / einsum.  ttmc_mode(X, factors, mode) is its
 Kronecker counterpart, the TTMc step of Tucker / HOOI, with the same inputs and a rank per mode.  tttp(X, factors)
 evaluates a CP model at X's stored entries (X * [[U_0, ..., U_{N-1}]], the order-N sddmm) and keeps X's pattern.
+ttm_mode(X, U, mode) is the mode-n tensor times matrix (or vector) with a sparse result: tensordot(X, U, axes=([mode],
+[0])) bit for bit, in O(nnz + result) memory instead of a dense intermediate over the other extents.
 
 masked_matmul(mask, a, b) == mask * (a @ b) at mask's stored positions, for sparse a and b: the masked SpGEMM of
 examples/triangles_example.py (sum(a @ a * a) / 6) and of the GraphBLAS masked mxm.  It never forms the product
@@ -137,11 +139,8 @@ def _mode_stream(X, mode):
     return stream
 
 
-def _tensor_and_factors(name, X, factors, mode, one_rank):
-    """Checks shared by mttkrp_mode, ttmc_mode and tttp: (order N, mode in 0..N-1, the factors as a list with the other
-    modes' ones as NumPy arrays or device tensors, the other modes ascending, the result dtype T, the ranks: a list of N
-    with ranks[m] = factors[m].shape[1] for the other modes and 0 for `mode`).  `mode` None (tttp) reads every factor.
-    With `one_rank` every factor read must have the same number of columns."""
+def _tensor_and_mode(name, X, mode):
+    """Checks of the tensor operand shared by the sparse-tensor ops: (order N, mode in 0..N-1, or None for None)."""
     from ._gcxs import GCXS
 
     if not isinstance(X, (COO, GCXS)):
@@ -155,6 +154,15 @@ def _tensor_and_factors(name, X, factors, mode, one_rank):
         if not -N <= mode < N:
             raise AxisError(mode, N)
         mode %= N
+    return N, mode
+
+
+def _tensor_and_factors(name, X, factors, mode, one_rank):
+    """Checks shared by mttkrp_mode, ttmc_mode and tttp: (order N, mode in 0..N-1, the factors as a list with the other
+    modes' ones as NumPy arrays or device tensors, the other modes ascending, the result dtype T, the ranks: a list of N
+    with ranks[m] = factors[m].shape[1] for the other modes and 0 for `mode`).  `mode` None (tttp) reads every factor.
+    With `one_rank` every factor read must have the same number of columns."""
+    N, mode = _tensor_and_mode(name, X, mode)
     factors = list(factors)
     if len(factors) != N:
         raise ValueError(f"{name}: {len(factors)} factors for an order-{N} tensor")
@@ -313,6 +321,125 @@ def tttp(X, factors):
     res = COO._from_device(X._dev()[0], out, X.shape, T.type(0), keys=X._keys)
     res._canonicalise(check_sort=False, sum_dups=False, prune=True)  # drops bitwise +0 results, as X * model does
     return res
+
+
+# Fibers with more entries than this get whole CTAs in b2s_ttm_mode (a module value so that tests can move it).
+_TTM_LONG_FIBER = 512
+
+
+def _long_fibers(X, mode, fptr):
+    """The ascending indices (int64) of the fibers of `mode` with more than _TTM_LONG_FIBER entries; cached next to the
+    fiber stream."""
+    key = ("fiber-long", mode, _index_limit(X) < 2**31 - 1, _TTM_LONG_FIBER)
+    if key not in X._mode_streams:
+        flags = Kn.ttm_mode_long_flags(fptr, _TTM_LONG_FIBER)
+        pos, n = Kn.scan_flags(flags)
+        X._mode_streams[key] = Kn.compact(Kn.iota(flags.shape[0]), flags, pos, n)
+    return X._mode_streams[key]
+
+
+def _fiber_stream(X, mode):
+    """The fiber stream of `mode` (the inputs of b2s_ttm_mode): (kcoord, vals, fptr, fgroup, gptr, fkey, pkey).
+
+    Entries are ordered by the key over the axes (other modes ascending, then `mode`): X's canonical order when `mode`
+    is the last axis, one stable sort otherwise.  Fibers (runs sharing every coordinate but `mode`) and groups (runs of
+    fibers sharing the coordinates before `mode`) come from the flag / scan / compact primitives.  Cached on X under
+    ("fiber", mode, int32 indices), apart from the mode streams of mttkrp_mode and dropped with them."""
+    from ._gcxs import GCXS
+    from ._utils import c_strides, key_bits
+
+    limit = _index_limit(X)
+    key = ("fiber", mode, limit < 2**31 - 1)
+    cache = X._mode_streams
+    if cache is not None and key in cache:
+        return cache[key]
+    c = X.tocoo() if isinstance(X, GCXS) else X
+    N, shape, nnz = X.ndim, X.shape, X.nnz
+    coords, vals = c._dev()
+    if mode == N - 1:
+        pc = coords  # canonical order is already the fiber stream's
+    else:
+        axes = [m for m in range(N) if m != mode] + [mode]
+        pshape = [shape[a] for a in axes]
+        strides = [0] * N
+        for a, s in zip(axes, c_strides(pshape)):
+            strides[a] = s
+        keys, perm = Kn.sort_keys(Kn.linearize(coords, strides), key_bits(X.size))
+        pc = Kn.unravel(keys, pshape, np.int64)  # rows: the other modes ascending, then `mode`
+        vals = Kn.gather(vals, perm)
+    fkey = Kn.linearize(pc[:N - 1], c_strides([shape[m] for m in range(N) if m != mode]))
+    pkey = Kn.linearize(pc[:mode], c_strides(shape[:mode])) if mode else Kn.full(nnz, 0, np.int64)
+    heads = Kn.flag_heads(fkey)
+    pos, nf = Kn.scan_flags(heads)
+    fstart = Kn.compact(Kn.iota(nnz), heads, pos, nf)
+    fkey, pkey = Kn.compact(fkey, heads, pos, nf), Kn.compact(pkey, heads, pos, nf)
+    gheads = Kn.flag_heads(pkey)
+    gpos, ng = Kn.scan_flags(gheads)
+    t = D.torch()
+    gptr = t.cat([Kn.compact(Kn.iota(nf), gheads, gpos, ng), Kn.full(1, nf, np.int64)])
+    fgroup = Kn.rows_from_indptr(gptr, nf, np.int64)
+    fptr = t.cat([fstart, Kn.full(1, nnz, np.int64)])
+    kc, fptr, fgroup, gptr = _narrow_idx(pc[N - 1].contiguous(), fptr, fgroup, gptr, limit=limit)
+    stream = (kc, vals, fptr, fgroup, gptr, fkey, pkey)
+    if cache is None:
+        cache = X._mode_streams = {}
+    cache[key] = stream
+    return stream
+
+
+def ttm_mode(X, U, mode):
+    """Mode-`mode` tensor times matrix (TTM) of a sparse tensor, ``X ×_mode Uᵀ``, with a sparse result; with a 1-D `U`,
+    tensor times vector (TTV).  The step of Tucker / HOSVD built from a chain of TTMs, of projecting a tensor onto a basis
+    along one mode, and of contracting one mode with a vector.
+
+        Y[i_0, ..., r, ..., i_{N-1}] = sum_{i_mode} X[i_0, ..., i_mode, ..., i_{N-1}] * U[i_mode, r]
+
+    `X` is a COO or GCXS of order 2..8 with a zero fill value; `mode` counts from the end when negative.  `U` is a NumPy
+    array or a CUDA tensor: 2-D of shape (X.shape[mode], R), R >= 0, gives X's shape with axis `mode` replaced by R;
+    1-D of shape (X.shape[mode],) gives X's shape with axis `mode` removed (order N - 1).  The dtype is
+    result_type(X.dtype, U.dtype), float32 or float64.  The result is always a canonical COO with fill value +0.  A
+    GCXS result is not offered: its indptr would span the product of the compressed extents, the size this op avoids.
+
+    The order of operations is fixed (include/sparse_b200.h, b2s_ttm_mode): each value is ((+0 + v_1 * U[k_1, r]) +
+    v_2 * U[k_2, r]) + ... over the mode-`mode` fiber's entries in ascending k, each product and sum rounded, and an
+    entry is stored iff its value != 0 (+-0 are dropped, NaN is kept).  So for a COO X the result equals
+    ``moveaxis(tensordot(X, U, axes=([mode], [0]), return_type=COO), -1, mode)`` (or the plain tensordot for a 1-D U)
+    bit for bit, wherever that fits in memory: tensordot builds an indptr over the product of the other extents and a
+    dense (that product x R) intermediate, where ttm_mode needs O(nnz + result).  For a GCXS X the result is
+    ``ttm_mode(X.tocoo(), U, mode)`` bit for bit; GCXS tensordot sums in float64 and agrees only to rounding.
+
+    Memory: the fiber stream of `mode` is cached on `X` for the next call with the same mode (dropped when X's contents
+    are replaced, not copied or pickled): nnz * (index bytes + value bytes) + n_fibers * (3 * index bytes + 16), index
+    bytes 4 when every extent and nnz fit int32, else 8, plus 8 bytes per fiber of more than 512 entries (such fibers
+    get whole thread blocks, so skewed fiber lengths do not hold up the rest).  During the call, n_fibers * R * (value bytes + 17) bytes of
+    slots before pruning, and the result, nnz(Y) * (value bytes + 8).  A result shape of 2**63 elements or more raises
+    ValueError before anything is allocated.
+    """
+    N, mode = _tensor_and_mode("ttm_mode", X, mode)
+    if not D.is_device_tensor(U):
+        U = np.asarray(U)
+    if U.ndim not in (1, 2) or int(U.shape[0]) != X.shape[mode]:
+        raise ValueError(f"ttm_mode: shape mismatch X{X.shape}, U {tuple(U.shape)} (expected ({X.shape[mode]},) or "
+                         f"({X.shape[mode]}, R) for mode {mode})")
+    T = np.result_type(X.dtype, _dense_dt(U))
+    if T not in (np.dtype("float32"), np.dtype("float64")):
+        raise TypeError(f"ttm_mode: dtype {T} is outside the CUDA dtype matrix (float32, float64)")
+    ttv = U.ndim == 1
+    R = 1 if ttv else int(U.shape[1])
+    shape = X.shape[:mode] + (() if ttv else (R,)) + X.shape[mode + 1:]
+    if int(np.prod(shape, dtype=object)) >= 2**63:
+        raise ValueError(f"ttm_mode: result shape {shape} has 2**63 elements or more (the COO index limit)")
+    if X.nnz == 0 or R == 0:
+        return COO._from_device(None, Kn.full(0, 0, T), shape, T.type(0), keys=Kn.full(0, 0, np.int64))
+    kc, vals, fptr, fgroup, gptr, fkey, pkey = _fiber_stream(X, mode)
+    long_ids = _long_fibers(X, mode, fptr)
+    q_ext = int(np.prod(X.shape[mode + 1:], dtype=object))
+    out, keys, flags = Kn.ttm_mode(kc, Kn.cast(vals, T), fptr, fgroup, gptr, fkey, pkey, long_ids, _TTM_LONG_FIBER,
+                                   _dense_dev(U.reshape(-1, 1) if ttv else U, T), R, q_ext)
+    pos, total = Kn.scan_flags(flags)
+    if total != int(out.shape[0]):
+        out, keys = Kn.compact(out, flags, pos, total), Kn.compact(keys, flags, pos, total)
+    return COO._from_device(None, out, shape, T.type(0), keys=keys)
 
 
 # Test hook: True keeps masked_matmul's index arrays int64 even when every extent and nnz fit int32.

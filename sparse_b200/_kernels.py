@@ -735,6 +735,42 @@ def tttp(coords, vals, factors, R):
 
 
 # ------------------------------------------------------------------------------------------------
+# K14 mode-n TTM
+# ------------------------------------------------------------------------------------------------
+def ttm_mode_long_flags(fptr, long_min):
+    """uint8 flags over the fibers of `fptr`: fiber f has more than long_min entries."""
+    t = _t()
+    nf = int(fptr.shape[0]) - 1
+    flags = t.empty(nf, dtype=t.uint8, device=fptr.device)
+    _lib.check(_lib.load().b2s_ttm_mode_long_flags(i32(_idx_bytes(fptr)), i64(nf), vp(D.ptr(fptr)), i64(long_min),
+                                                   vp(D.ptr(flags)), _sp()), "b2s_ttm_mode_long_flags")
+    return flags
+
+
+def ttm_mode(kcoord, vals, fptr, fgroup, gptr, fkey, pkey, long_ids, long_min, U, R, q_ext):
+    """(values, keys, keep flags) of the n_fibers * R slots of mode-n TTM over a fiber stream, in the fixed order of
+    b2s_ttm_mode: y(f, r) = sum over fiber f's entries in stream order of vals[e] * U[kcoord[e], r], at slot
+    R * g0 + r * s_g + (f - g0) with key (P * R + r) * q_ext + Q, flag y != 0.  `kcoord`, `fptr`, `fgroup` and `gptr`
+    share one index width; `fkey` / `pkey` are int64; `long_ids` (int64) lists exactly the fibers with more than
+    `long_min` entries (ttm_mode_long_flags); U is (rows, R)."""
+    t = _t()
+    nf = int(fkey.shape[0])
+    assert fptr.dtype == kcoord.dtype and fgroup.dtype == kcoord.dtype and gptr.dtype == kcoord.dtype
+    _, fptrs, ld, keep = _factor_args([kcoord], vals, [U], [R])
+    n = nf * int(R)
+    out = t.empty(n, dtype=vals.dtype, device=vals.device)
+    keys = t.empty(n, dtype=t.int64, device=vals.device)
+    flags = t.empty(n, dtype=t.uint8, device=vals.device)
+    rc = _lib.load().b2s_ttm_mode(i32(D.dtype_code(D.np_dtype(vals))), i32(_idx_bytes(kcoord)), i64(nf), i64(R),
+                                  i64(q_ext), vp(D.ptr(kcoord)), vp(D.ptr(vals)), vp(D.ptr(fptr)), vp(D.ptr(fgroup)),
+                                  vp(D.ptr(gptr)), vp(D.ptr(fkey)), vp(D.ptr(pkey)), vp(D.ptr(long_ids)),
+                                  i64(long_ids.shape[0]), i64(long_min), vp(fptrs[0]), i64(ld[0]),
+                                  vp(D.ptr(out)), vp(D.ptr(keys)), vp(D.ptr(flags)), _sp())
+    _lib.check(rc, "b2s_ttm_mode")
+    return out, keys, flags
+
+
+# ------------------------------------------------------------------------------------------------
 # K11 masked SpGEMM
 # ------------------------------------------------------------------------------------------------
 def masked_spgemm(m_indptr, m_cols, m_vals, a_indptr, a_cols, a_vals, bt_indptr, bt_cols, bt_vals, M, N, K):

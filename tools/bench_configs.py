@@ -5,10 +5,10 @@ Device-resident inputs (generated with seeded torch generators on the GPU), wall
 torch.cuda.synchronize() because the public calls contain their own size-returning syncs.
 Prints one line per config as it runs and the whole result as one JSON line at the end.
 
-    python tools/bench_configs.py [c1 c3 c3big red c4 c5 mttkrp mttkrp_mode masked ttmc tttp]
+    python tools/bench_configs.py [c1 c3 c3big red c4 c5 mttkrp mttkrp_mode masked ttmc tttp ttm]
 
-`masked` (the masked SpGEMM, examples/triangles_example.py), `ttmc` (the Tucker / HOOI step) and `tttp` (a CP model at
-a sparse tensor's entries) run only when named.
+`masked` (the masked SpGEMM, examples/triangles_example.py), `ttmc` (the Tucker / HOOI step), `tttp` (a CP model at
+a sparse tensor's entries) and `ttm` (mode-n tensor times matrix with a sparse result) run only when named.
 """
 import json
 import os
@@ -283,6 +283,8 @@ def run(which=None, compact=False, parity=True):
         res.update(_ttmc(rec, parity))
     if "tttp" in which:
         res.update(_tttp(rec, parity))
+    if "ttm" in which:
+        res.update(_ttm(rec, parity))
     torch.cuda.empty_cache()
     return res
 
@@ -723,6 +725,191 @@ def _tttp(rec, parity):
     r["unfused"] = unf
     out[name] = r
     del Bk, U, got
+    torch.cuda.empty_cache()
+    return out
+
+
+def _ttm_models(X, nf, R, vb=4, ib=4):
+    """Byte model of one ttm_mode call with the fiber stream cached (f32, int32 indices): the stream (entries, and per
+    fiber its pointer, group, key and P key), one R-column row of U per entry counted as if every gather came from HBM
+    (most are L2 hits), the n_fibers * R slots (value, key, flag) and the scan over the flags (read, positions)."""
+    nnz = X.nnz
+    b = {"stream": nnz * (ib + vb) + nf * (2 * ib + 16), "u_gathers": nnz * R * vb, "slots": nf * R * (vb + 9),
+         "scan": nf * R * 9}
+    b["total"] = sum(b.values())
+    return {"bytes": b, "model_ms_bytes_at_3.35TBs": round(b["total"] / 3.35e12 * 1e3, 3)}
+
+
+def _ttm_parity(X, U, mode, got, samples, seed):
+    """Every value against an fp64 device restatement (per-fiber index_add of v * U[k], rtol 2e-5), and `samples`
+    sampled fibers bit-compared with the CPU restatement of the order (tests/_ttm_order.py)."""
+    import _ttm_order as TO
+
+    coords, vals = X._dev()
+    shape, N = X.shape, X.ndim
+    others = [m for m in range(N) if m != mode]
+
+    def fiber_keys(c):
+        k = torch.zeros(c.shape[1], dtype=torch.int64, device=DEV)
+        for m in others:
+            k = k * shape[m] + c[m].to(torch.int64)
+        return k
+
+    Ud = U.double()
+    fk = fiber_keys(coords)
+    uk, inv = torch.unique(fk, return_inverse=True)
+    del fk
+    want = torch.zeros((uk.numel(), Ud.shape[1]), dtype=torch.float64, device=DEV)
+    mag = torch.zeros_like(want)  # sum of |v * U| per (fiber, r): the scale of the f32 rounding error
+    step = 20_000_000
+    for s in range(0, X.nnz, step):
+        prod = vals[s:s + step].double()[:, None] * Ud[coords[mode, s:s + step]]
+        want.index_add_(0, inv[s:s + step], prod)
+        mag.index_add_(0, inv[s:s + step], prod.abs())
+        del prod
+    # a serial sum of L rounded f32 products is within (L + 1) * 2**-24 * sum |v * U| of the exact one (the standard
+    # recursive-summation bound); long fibers can exceed a plain rtol, so each value gets the larger of the two
+    flen = torch.bincount(inv, minlength=uk.numel()).double()
+    del inv
+    R = Ud.shape[1]
+    q_ext = int(np.prod(shape[mode + 1:], dtype=np.int64))
+    keys, gv = got.sorted_keys(), got._data_dev()
+    close, gfk_parts = True, []
+    for s in range(0, got.nnz, step):
+        k = keys[s:s + step]
+        r = torch.div(k, q_ext, rounding_mode="floor") % R
+        gfk = torch.div(k, q_ext * R, rounding_mode="floor") * q_ext + k % q_ext
+        gfk_parts.append(gfk)
+        fi = torch.searchsorted(uk, gfk)
+        w = want[fi, r]
+        tol = torch.maximum(2e-5 * w.abs(), (flen[fi] + 1) * 2.0**-24 * mag[fi, r])
+        close &= bool(((gv[s:s + step].double() - w).abs() <= tol).all())
+    del want, mag, flen
+    pick = torch.from_numpy(np.sort(np.random.default_rng(seed).choice(uk.numel(), samples, replace=False))).to(DEV)
+    chosen = uk[pick]
+    sel = torch.isin(fiber_keys(coords), chosen)
+    gsel = torch.isin(torch.cat(gfk_parts), chosen)
+    rc, rv = TO.result(coords[:, sel].cpu().numpy(), vals[sel].cpu().numpy(), shape, U.cpu().numpy(), mode,
+                       np.float32)
+    got_c = torch.stack(torch.unravel_index(keys[gsel], got.shape)).cpu().numpy()
+    exact = bool(np.array_equal(got_c, rc) and TO.same_bits(gv[gsel].cpu().numpy(), rv))
+    return {"vs": f"fp64 device restatement (all values, within max(rtol 2e-5, (L + 1) * 2**-24 * sum |v * U|) for a "
+                  f"fiber of L entries) + {samples} sampled fibers bit-compared with the CPU restatement of the order "
+                  "(tests/_ttm_order.py)",
+            "values_close": close, "sampled_fibers_bit_exact": exact}
+
+
+def _ttm_vs_tensordot(name, X, mode, R, seed, card, parity):
+    """ttm_mode against moveaxis(tensordot(..., return_type=COO), -1, mode), alternating, median of 5 each, and the peak
+    device memory of one call of each beyond the inputs; ttm_mode's first call is measured, so its peak includes
+    building the fiber stream that then stays cached on X."""
+    g = torch.Generator(device=DEV).manual_seed(seed)
+    U = torch.rand((X.shape[mode], R), generator=g, device=DEV, dtype=torch.float32)
+    fns = {"ttm_mode": lambda: sp.ttm_mode(X, U, mode),
+           "tensordot": lambda: sp.moveaxis(sp.tensordot(X, U, axes=([mode], [0]), return_type=sp.COO), -1, mode)}
+    peak = {}
+    for k, fn in fns.items():
+        X._mode_streams = None
+        fn()  # warms the kernels; for tensordot, also the first call's allocations
+        X._mode_streams = None
+        torch.cuda.synchronize()
+        torch.cuda.reset_peak_memory_stats(DEV)
+        base = torch.cuda.memory_allocated(DEV)
+        fn()
+        torch.cuda.synchronize()
+        peak[k] = int(torch.cuda.max_memory_allocated(DEV) - base)
+    times = {k: [] for k in fns}
+    for _ in range(5):
+        for k, fn in fns.items():
+            times[k].append(timeit(fn, reps=1, warm=0)[0])
+    got, want = fns["ttm_mode"](), fns["tensordot"]()
+    nf = int(X._mode_streams[("fiber", mode, True)][5].numel())
+    r = {"ms_median": round(float(np.median(times["ttm_mode"])), 4), "ms_best": round(min(times["ttm_mode"]), 4),
+         "tensordot_ms_median": round(float(np.median(times["tensordot"])), 4),
+         "tensordot_ms_best": round(min(times["tensordot"]), 4),
+         "speedup_vs_tensordot": round(float(np.median(times["tensordot"]) / np.median(times["ttm_mode"])), 2),
+         "peak_extra_bytes_incl_fiber_stream": peak["ttm_mode"], "tensordot_peak_extra_bytes": peak["tensordot"],
+         "card": card, "n_fibers": nf, **_ttm_models(X, nf, R)}
+    if parity:
+        gb, wb = got._data_dev(), want._data_dev()
+        r["parity"] = _ttm_parity(X, U, mode, got, 2_000, seed + 1)
+        r["parity"]["whole_result_bit_exact_vs_tensordot"] = bool(
+            got.nnz == want.nnz and torch.equal(got.sorted_keys(), want.sorted_keys())
+            and torch.equal(gb.view(torch.int32), wb.view(torch.int32)))
+    print(name, r, flush=True)
+    return r
+
+
+def _ttm(rec, parity):
+    """Mode-n TTM with a sparse result: short fibers (about one entry each, the output-write bound regime) at modes 0
+    and 2, long fibers (about 100 entries, U gathers mostly L2 hits), and two shapes where tensordot still fits -- one
+    uniform, one with Zipf fiber lengths up to 1e6 entries -- timed against it alternating, with both calls' peak extra
+    device memory."""
+    sys.path.insert(0, os.path.join(ROOT, "tests"))
+    import _ttm_order as TO
+
+    out = {}
+    card = _card()
+    cases = (("short fibers (1e6,1e6,100) nnz 1e8", (1_000_000, 1_000_000, 100), (0, 2), 8, 91),
+             ("long fibers (1e3,1e3,1e5) nnz 1e8", (1_000, 1_000, 100_000), (2,), 64, 93))
+    for label, shape, modes, R, seed in cases:
+        X = rand_coo(shape, 100_000_000, seed, torch.float32)
+        g = torch.Generator(device=DEV).manual_seed(seed + 1)
+        for mode in modes:
+            U = torch.rand((shape[mode], R), generator=g, device=DEV, dtype=torch.float32)
+            torch.cuda.synchronize()
+            X._mode_streams = None
+            t0 = time.perf_counter()
+            got = sp.ttm_mode(X, U, mode)
+            torch.cuda.synchronize()
+            first = (time.perf_counter() - t0) * 1e3
+            nf = int(X._mode_streams[("fiber", mode, True)][5].numel())
+            models = _ttm_models(X, nf, R)
+            name = f"ttm_mode {label} mode {mode} R={R} f32"
+            r = rec(name, lambda: sp.ttm_mode(X, U, mode), X.nnz, "Gnnz_s", models["bytes"]["total"])
+            r.update({"card": card, "first_call_ms_incl_fiber_stream": round(first, 3), "n_fibers": nf,
+                      "out_nnz": got.nnz, **models})
+            if parity:
+                r["parity"] = _ttm_parity(X, U, mode, got, 2_000, seed + 2)
+            out[name] = r
+            del got, U
+            X._mode_streams = None
+            torch.cuda.empty_cache()
+        del X
+        torch.cuda.empty_cache()
+
+    # tensordot still fits: fused against unfused, alternating, with the peak extra memory of each
+    shape, mode, R = (10_000, 1_000, 1_000), 2, 16
+    X = rand_coo(shape, 10_000_000, 95, torch.float32)
+    name = "ttm_mode (1e4,1e3,1e3) nnz 1e7 mode 2 R=16 f32 vs tensordot(return_type=COO)"
+    out[name] = _ttm_vs_tensordot(name, X, mode, R, 96, card, parity)
+    del X
+    torch.cuda.empty_cache()
+
+    # skewed fiber lengths (Zipf, the longest 1e6 entries) where tensordot still fits
+    shape, mode, R = (10_000, 1_000, 2_000_000), 2, 8
+    g = torch.Generator(device=DEV).manual_seed(98)
+    size = int(np.prod(shape))
+    parts = [torch.randint(0, size, (20_000_000,), generator=g, device=DEV)]
+    fibers = torch.randint(0, shape[0] * shape[1], (4_000,), generator=g, device=DEV).tolist()
+    for i, fib in enumerate(fibers, start=1):
+        n = int(1e6 * i ** -1.2)
+        if n < 64:
+            break
+        parts.append(fib * shape[2] + torch.randint(0, shape[2], (n,), generator=g, device=DEV))
+    lin = torch.cat(parts)
+    del parts
+    X = sp.COO(torch.stack(torch.unravel_index(lin, shape)), torch.rand(lin.numel(), generator=g, device=DEV),
+               shape=shape)  # duplicates summed, sorted
+    del lin
+    name = "ttm_mode skewed fibers (1e4,1e3,2e6) nnz 2.6e7 Zipf lengths up to 1e6, mode 2 R=8 f32 vs tensordot"
+    r = _ttm_vs_tensordot(name, X, mode, R, 99, card, parity)
+    fp = X._mode_streams[("fiber", mode, True)][2].to(torch.int64)
+    lens = fp[1:] - fp[:-1]
+    r.update({"nnz": X.nnz, "longest_fiber": int(lens.max()), "fibers_over_512": int((lens > 512).sum()),
+              "entries_in_fibers_over_512": int(lens[lens > 512].sum())})
+    out[name] = r
+    del X, fp, lens
     torch.cuda.empty_cache()
     return out
 

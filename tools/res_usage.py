@@ -20,7 +20,8 @@ HOT = [r"spmm_csr_dense_dyn_kernel<float, int, 4, 32, 8, 4>", r"spmm_csr_dense_d
        r"rd_emit_kernel<float", r"reduce_tile_kernel<double", r"sddmm_kernel<float", r"mttkrp_kernel<float", r"mttkrp_mode_kernel<float", r"mttkrp_combine_kernel<float",
        r"ttmc_mode_kernel<float, int, 4, 16, 8>", r"ttmc_mode_kernel<float, int, 1, 16, 8>",
        r"ttmc_mode_kernel<double, int, 2, 16, 8>", r"tttp_kernel<float, int, 4>", r"tttp_kernel<float, int, 1>",
-       r"tttp_kernel<double, int, 2>",
+       r"tttp_kernel<double, int, 2>", r"ttm_mode_kernel<float, int, 4>", r"ttm_mode_kernel<float, int, 1>",
+       r"ttm_mode_kernel<double, int, 2>",
        r"masked_spgemm_kernel<float, float, int, 32>", r"masked_spgemm_kernel<double, double, int, 8>",
        r"spmm_bulk_kernel<float"]
 
