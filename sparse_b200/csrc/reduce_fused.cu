@@ -56,10 +56,33 @@ __device__ __forceinline__ T red_apply(int op, T a, T b) {
     }
 }
 
-// fill-value contribution of SparseArray.reduce (_sparse_array.py:405-422)
+// fill-value contribution of SparseArray.reduce (_sparse_array.py:405-422).  NumPy computes fill (T) * n_fill (int64)
+// and fill ** n_fill in float64 and combines them with v in float64 too, rounding to T once: for float32 the whole step
+// runs in double here, unfused, so that add is bit-identical to it (and a contribution that overflows or underflows
+// float32 on its own, such as 3e38 * 2 or 0.5 ** 150, still reaches the result correctly).
+// b ** n for n > 0.  CUDA's pow may be an ulp or two off even where the result is exact, so a power of two base
+// (fill 0.5, 2, -4, ...) is raised exactly by its exponent; that keeps results such as 0.5 * 0.5 ** 6 equal to the
+// result fill 0.5 ** 7, and so pruned, as NumPy's correctly rounded pow does.
+__device__ __forceinline__ double fill_pow(double b, int64_t n) {
+    int e;
+    const double m = frexp(b, &e);
+    if (fabs(m) == 0.5) {
+        // |e - 1| <= 1074, and any |k| >= 4096 already gives inf or 0: clamp n first so that k cannot overflow
+        const int k = (e - 1) * (int)(n > 4096 ? 4096 : n);
+        const double r = ldexp(1.0, k);
+        // the sign follows NumPy's float64 exponent: from 2^53 on, (double)n is even
+        return (m < 0 && n < (1ll << 53) && (n & 1)) ? -r : r;
+    }
+    return pow(b, (double)n);
+}
+
 template <typename T>
 __device__ __forceinline__ T fill_fix(int op, T v, int64_t count, int64_t ncols, T fill) {
     const int64_t nf = ncols - count;
+    if constexpr (std::is_same<T, float>::value) {
+        if (op == RF_ADD) return (float)__dadd_rn((double)v, nf != 0 ? __dmul_rn((double)fill, (double)nf) : 0.0);
+        if (op == RF_MUL) return (float)__dmul_rn((double)v, nf != 0 ? fill_pow((double)fill, nf) : 1.0);
+    }
     if (op == RF_ADD) {
         T contrib = T(0);
         if (nf != 0) {
@@ -71,7 +94,7 @@ __device__ __forceinline__ T fill_fix(int op, T v, int64_t count, int64_t ncols,
     if (op == RF_MUL) {
         T contrib = T(1);
         if (nf != 0) {
-            if constexpr (std::is_floating_point<T>::value) contrib = (T)pow((double)fill, (double)nf);
+            if constexpr (std::is_floating_point<T>::value) contrib = (T)fill_pow((double)fill, nf);
             else {
                 T b = fill, r = T(1);
                 int64_t e = nf;

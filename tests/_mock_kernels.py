@@ -423,12 +423,12 @@ def reduce_fill_fix(op, vals, counts, ncols, fill_value):
     nf = ncols - c
     fill = v.dtype.type(fill_value)
     with np.errstate(all="ignore"):
-        if op == 0:
-            contrib = np.where(nf == 0, v.dtype.type(0), np.multiply(fill, nf).astype(v.dtype))
-            v[:] = (v + contrib).astype(v.dtype)
-        elif op == 1:
-            contrib = np.where(nf == 0, v.dtype.type(1), np.power(fill, nf).astype(v.dtype))
-            v[:] = (v * contrib).astype(v.dtype)
+        if op in (0, 1):
+            # contribution and combine in the type NumPy promotes T and int64 n_fill to (float64 for float32, int64 for
+            # the integers), rounded to T once at the end, as _sparse_array.py:410-421 does
+            method, sup, identity = (np.add, np.multiply, 0) if op == 0 else (np.multiply, np.power, 1)
+            contrib = np.where(nf == 0, identity, sup(fill, nf))
+            v[:] = method(v, contrib).astype(v.dtype)
         else:
             m = nf != 0
             v[m] = _RED[op](v[m], fill).astype(v.dtype)
