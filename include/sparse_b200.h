@@ -345,6 +345,39 @@ int b2s_ttmc_mode(int dtype, int idx_bytes, int order, int mode, int64_t nnz, in
                   const void *const *coords_host, const void *vals_dev, const void *const *factors_host,
                   const int64_t *ld_host, void *out_dev, int64_t ldo, void *stream);
 
+/* ---- the row-wise regularised least-squares ALS update of CP tensor completion, mode n of a sparse tensor of order
+ * 2..8 (K15, cp_completion.cu; no reference counterpart) ------------------------------------------------------------
+ * out[i, :] = x with (G_i + reg I) x = b_i, G_i = sum_e h_e h_e^T and b_i = sum_e v_e h_e over the stored entries e with
+ * i_mode(e) = i, h_e[r] = prod_{m != mode} U_m[i_m(e), r].  Arguments as b2s_mttkrp_mode (the same MODE STREAM S_mode,
+ * factors of R columns, entry `mode` never read); reg is finite and >= 0 and is cast to the value type;
+ * R <= B2S_CP_COMPLETION_MAX_RANK.  out is dense (rows x R, row stride ldo), fully written.  Scratch: two slots of
+ * R(R+1)/2 + R values per chunk for the rows that cross chunks.  No atomics, no stream synchronisation.
+ *
+ * Fixed order of operations (results are reproducible bit for bit, whatever the grid, SM count, index width, stream or
+ * gather path); every operation is rounded separately, no FMA contraction:
+ *  1. The input is the mode stream S_mode, cut into chunks of B2S_MTTKRP_CHUNK entries, as b2s_mttkrp_mode's steps 1
+ *     and 3.
+ *  2. For each entry e, over the other modes a < b < ... ascending: p_e[r] = ((v_e * U_a[i_a, r]) * U_b[i_b, r]) * ...
+ *     (b2s_mttkrp_mode's step 2), h_e[r] = (U_a[i_a, r] * U_b[i_b, r]) * ..., and g_e[r, s] = h_e[r] * h_e[s] for r <= s.
+ *  3. b_i (from p_e) and the upper triangle of G_i (from g_e) are summed as b2s_mttkrp_mode's steps 4 and 5: per
+ *     (chunk, row) ((+0 + x_1) + x_2) + ... in stream order, then ((+0 + partial_c1) + partial_c2) + ... in chunk
+ *     order.  So b_i is b2s_mttkrp_mode's row i bit for bit.
+ *  4. A = G_i with A[r, r] = G_i[r, r] + reg; the lower triangle mirrors the upper.
+ *  5. Cholesky, j = 0 .. R-1 in order: d = ((A_jj - L_j0 * L_j0) - L_j1 * L_j1) - ..., k ascending below j.  If !(d > 0)
+ *     the row fails and is written as NaN.  Else L_jj = sqrt(d), correctly rounded, and for i > j
+ *     L_ij = (((A_ij - L_i0 * L_j0) - L_i1 * L_j1) - ...) / L_jj.
+ *  6. y_j = ((b_j - L_j0 * y_0) - L_j1 * y_1 - ...) / L_jj, j ascending, k ascending.
+ *  7. x_j = ((y_j - L_{j+1,j} * x_{j+1}) - L_{j+2,j} * x_{j+2} - ...) / L_jj, j descending, k ascending from j + 1;
+ *     out[i, :] = x.
+ * A row without entries is the solution of reg I x = 0: +0 for reg > 0, NaN for reg = 0 (step 5 fails).
+ */
+#define B2S_CP_COMPLETION_MAX_RANK 64
+int b2s_cp_completion_max_rank(void); /* returns B2S_CP_COMPLETION_MAX_RANK */
+int b2s_cp_completion_mode(int dtype, int idx_bytes, int order, int mode, int64_t nnz, int64_t rows, int64_t R,
+                           double reg, const void *const *coords_host, const void *vals_dev,
+                           const void *const *factors_host, const int64_t *ld_host, void *out_dev, int64_t ldo,
+                           void *stream);
+
 /* ---- a sparse tensor of order 2..8 times a CP model at its stored entries (K13, tttp.cu; TTTP, the order-N SDDMM,
  * no reference counterpart) ------------------------------------------------------------------------------------------
  * out_vals[e] = v_e * sum_r U_0[i_0(e), r] * U_1[i_1(e), r] * ... * U_{order-1}[i_{order-1}(e), r] for each of the nnz

@@ -323,6 +323,62 @@ def tttp(X, factors):
     return res
 
 
+def cp_completion_mode(X, factors, mode, reg):
+    """One ALS update of CP tensor completion: the new factor of mode `mode`, each row the solution of its own
+    regularised least-squares problem over the entries observed in that row.
+
+        h_e[r] = prod_{m != mode} factors[m][i_m(e), r]           (the Khatri-Rao row of entry e)
+        (sum_{e in row i} h_e h_e^T + reg * I) u_i = sum_{e in row i} v_e h_e,      out[i] = u_i
+
+    `X` is a COO or GCXS of order 2..8 with a zero fill value; its stored entries are the observed set, stored zeros
+    included (a COO built with the default ``prune=False`` keeps them, and they count as observations of 0).
+    `factors` is as for `mttkrp_mode`: N dense 2-D arrays (NumPy arrays or CUDA tensors, which may be mixed),
+    `factors[m]` of shape (X.shape[m], R) with one R for all; `factors[mode]` is not read and may be None.  `reg` is a
+    finite real >= 0, cast to the result dtype.  The result is dense, (X.shape[mode], R), of dtype
+    result_type(X.dtype, other factor dtypes) (float32 or float64): a NumPy array, or a CUDA tensor when a factor is
+    one.  R is at most `_kernels.cp_completion_max_rank()` (64); a larger R raises ValueError before anything is
+    allocated.
+
+    A row without entries is the solution of reg * I u = 0: zero for reg > 0, NaN for reg = 0.  A row whose
+    Cholesky factorisation meets a pivot that is not positive (a rank-deficient row at reg = 0, or NaN / inf inputs)
+    comes back as all NaN; the other rows are unaffected.
+
+    The order of operations is fixed (include/sparse_b200.h, b2s_cp_completion_mode), so results are reproducible bit
+    for bit; the right-hand side sum_e v_e h_e is `mttkrp_mode(X, factors, mode)[i]` bit for bit.
+
+    An ALS sweep, with `tttp` for the training loss:
+
+        for it in range(sweeps):
+            for n in range(X.ndim):
+                U[n] = cp_completion_mode(X, U, n, reg)
+            P = COO(X.coords, np.ones(X.nnz), shape=X.shape)             # X's pattern with ones
+            resid = tttp(P, U) - X
+            loss = 0.5 * (resid.data ** 2).sum() + 0.5 * reg * sum((u ** 2).sum() for u in U)
+
+    Memory: the mode stream of `mode`, cached on `X` and shared with `mttkrp_mode` (not rebuilt); the result,
+    rows * R * itemsize; and, during the call, a scratch array of 2 * ceil(nnz / 512) * W * itemsize bytes
+    (W = R(R+1)/2 + R rounded up to a multiple of 4) for the rows that cross chunks.  No (rows, R^2) array is formed.
+    """
+    N, mode, factors, T, ranks = _tensor_and_factors("cp_completion_mode", X, factors, mode, True)
+    R = max(ranks)
+    if isinstance(reg, (bool, np.bool_)) or not isinstance(reg, (int, float, np.integer, np.floating)):
+        raise TypeError(f"cp_completion_mode: `reg` must be a real number, got {type(reg).__name__}")
+    with np.errstate(over="ignore"):
+        reg_t = T.type(reg)
+    if not np.isfinite(reg_t) or reg_t < 0:
+        raise ValueError(f"cp_completion_mode: `reg` must be finite and >= 0 in {T}, got {reg!r}")
+    if R > Kn.cp_completion_max_rank():
+        raise ValueError(f"cp_completion_mode: R = {R} exceeds the limit of {Kn.cp_completion_max_rank()}")
+    rows = X.shape[mode]
+    if X.nnz == 0 or rows == 0 or R == 0:
+        out = Kn.full(rows * R, 0 if reg_t > 0 else np.nan, T).reshape(rows, R)
+    else:
+        coords, vals = _mode_stream(X, mode)
+        fac = [None if m == mode else _dense_dev(factors[m], T) for m in range(N)]
+        out = Kn.cp_completion_mode(coords, Kn.cast(vals, T), fac, mode, rows, R, float(reg_t))
+    return _return_dense(out, [f for f in factors if f is not None])
+
+
 # Fibers with more entries than this get whole CTAs in b2s_ttm_mode (a module value so that tests can move it).
 _TTM_LONG_FIBER = 512
 

@@ -735,6 +735,29 @@ def tttp(coords, vals, factors, R):
 
 
 # ------------------------------------------------------------------------------------------------
+# K15 CP completion (row-wise regularised least squares)
+# ------------------------------------------------------------------------------------------------
+def cp_completion_max_rank() -> int:
+    """Largest R that b2s_cp_completion_mode accepts (B2S_CP_COMPLETION_MAX_RANK)."""
+    return int(_lib.load().b2s_cp_completion_max_rank())
+
+
+def cp_completion_mode(coords, vals, factors, mode, rows, R, reg):
+    """out[i] = x with (G_i + reg I) x = b_i over the stream entries e with coords[mode][e] = i (G_i = sum h_e h_e^T,
+    b_i = sum vals[e] h_e, h_e the Khatri-Rao row of the other factors), in the fixed order of b2s_cp_completion_mode.
+    `coords` (N index tensors, one width) and `vals` are the mode stream; factors[mode] is not read; `reg` is a
+    Python float already rounded to the value type."""
+    N = len(coords)
+    ptrs, fptrs, ld, keep = _factor_args(coords, vals, factors, [R] * N, mode)
+    out = _t().empty((rows, R), dtype=vals.dtype, device=vals.device)
+    rc = _lib.load().b2s_cp_completion_mode(i32(D.dtype_code(D.np_dtype(vals))), i32(_idx_bytes(coords[0])), i32(N),
+                                            i32(mode), i64(vals.shape[0]), i64(rows), i64(R), ctypes.c_double(reg),
+                                            ptrs, vp(D.ptr(vals)), fptrs, ld, vp(D.ptr(out)), i64(R), _sp())
+    _lib.check(rc, "b2s_cp_completion_mode")
+    return out
+
+
+# ------------------------------------------------------------------------------------------------
 # K14 mode-n TTM
 # ------------------------------------------------------------------------------------------------
 def ttm_mode_long_flags(fptr, long_min):

@@ -5,10 +5,11 @@ Device-resident inputs (generated with seeded torch generators on the GPU), wall
 torch.cuda.synchronize() because the public calls contain their own size-returning syncs.
 Prints one line per config as it runs and the whole result as one JSON line at the end.
 
-    python tools/bench_configs.py [c1 c3 c3big red c4 c5 mttkrp mttkrp_mode masked ttmc tttp ttm]
+    python tools/bench_configs.py [c1 c3 c3big red c4 c5 mttkrp mttkrp_mode masked ttmc tttp ttm completion]
 
 `masked` (the masked SpGEMM, examples/triangles_example.py), `ttmc` (the Tucker / HOOI step), `tttp` (a CP model at
-a sparse tensor's entries) and `ttm` (mode-n tensor times matrix with a sparse result) run only when named.
+a sparse tensor's entries), `ttm` (mode-n tensor times matrix with a sparse result) and `completion` (the ALS update
+of CP tensor completion) run only when named.
 """
 import json
 import os
@@ -285,6 +286,8 @@ def run(which=None, compact=False, parity=True):
         res.update(_tttp(rec, parity))
     if "ttm" in which:
         res.update(_ttm(rec, parity))
+    if "completion" in which:
+        res.update(_completion(rec, parity))
     torch.cuda.empty_cache()
     return res
 
@@ -910,6 +913,139 @@ def _ttm(rec, parity):
               "entries_in_fibers_over_512": int(lens[lens > 512].sum())})
     out[name] = r
     del X, fp, lens
+    torch.cuda.empty_cache()
+    return out
+
+
+def _completion_models(X, mode, R, vb=4, ib=4):
+    """Models of one cp_completion_mode call (f32, int32 coordinates).  Bytes: the mode stream, one R-column row of
+    every other factor per entry counted as if every gather came from HBM (K10's model), the result, and the crossing
+    rows' scratch written and read.  Operations: R(R+1)/2 multiplies and as many adds per entry, R of each for b, and
+    about R^3 / 3 per row for the factorisation and the solves, against 132 SMs x 128 FP32 lanes x 1.98 GHz without
+    FMA (33.4 Tops/s: a multiply and an add are two instructions)."""
+    N, nnz, rows = X.ndim, X.nnz, X.shape[mode]
+    ns = R * (R + 1) // 2 + R
+    nchunks = -(-nnz // 512)
+    b = {"stream": nnz * (N * ib + vb), "factor_gathers": nnz * (N - 1) * R * vb, "output": rows * R * vb,
+         "crossing_scratch": 2 * 2 * nchunks * ((ns + 3) // 4 * 4) * vb}
+    b["total"] = sum(b.values())
+    ops = {"entries": nnz * 2 * ns, "rows": int(rows * R ** 3 / 3 * 2)}
+    ops["total"] = sum(ops.values())
+    return {"bytes": b, "model_ms_bytes_at_3.35TBs": round(b["total"] / 3.35e12 * 1e3, 3), "ops": ops,
+            "model_ms_ops_at_33.4Tops": round(ops["total"] / 33.4e12 * 1e3, 3)}
+
+
+def _completion_parity(X, U, mode, R, reg, got, sample_rows, seed):
+    """Every row against an fp64 device solve of (G_i + reg I) x = b_i (G and b summed in fp64), and `sample_rows`
+    rows bit-compared with the CPU restatement of the order (tests/_completion_order.py)."""
+    import _completion_order as CO
+
+    coords, vals = X._dev()
+    rows = X.shape[mode]
+    others = [m for m in range(X.ndim) if m != mode]
+    iu = torch.triu_indices(R, R, device=DEV)
+    G = torch.zeros((rows, R, R), dtype=torch.float64, device=DEV)
+    b = torch.zeros((rows, R), dtype=torch.float64, device=DEV)
+    for s in range(0, X.nnz, 2_000_000):
+        c = coords[:, s:s + 2_000_000]
+        h = U[others[0]][c[others[0]]].double()
+        for m in others[1:]:
+            h = h * U[m][c[m]].double()
+        G.index_put_((c[mode],), h[:, :, None] * h[:, None, :], accumulate=True)
+        b.index_add_(0, c[mode], vals[s:s + 2_000_000].double()[:, None] * h)
+        del h
+    G += reg * torch.eye(R, dtype=torch.float64, device=DEV)
+    want = torch.linalg.solve(G, b)
+    del G, b
+    err = ((got.double() - want).abs().amax(1) / want.abs().amax(1).clamp_min(1e-30))
+    close = bool((err <= 1e-3).all())
+    worst = float(err.max())
+    del want, err
+    (sc, sv) = X._mode_streams[(mode, True)]
+    rowc = sc[mode]
+    pick = np.sort(np.random.default_rng(seed).choice(rows, sample_rows, replace=False))
+    bounds = torch.searchsorted(rowc, torch.from_numpy(np.stack([pick, pick + 1])).to(DEV).to(rowc.dtype)).cpu().numpy()
+    Gu, bb = [], []
+    for lo, hi in zip(bounds[0], bounds[1]):
+        gathered = [U[m][sc[m][lo:hi].long()].cpu().numpy() for m in others]
+        h, p = CO.khatri_rao(sv[lo:hi].cpu().numpy(), gathered, np.float32)
+        gu, bi = CO.row_system(h, p, int(lo), 512, np.float32)
+        Gu.append(gu)
+        bb.append(bi)
+    want_rows = CO.solve(np.array(Gu), np.array(bb), np.float32(reg), np.float32)
+    return {"vs": f"fp64 device solve of every row (max |x - x64| / max |x64| <= 1e-3) + {sample_rows} sampled rows "
+                  "bit-compared with the CPU restatement of the order (tests/_completion_order.py)",
+            "values_close": close, "worst_row_rel_err": worst,
+            "sampled_rows_bit_exact": CO.same_bits(got[torch.from_numpy(pick).to(DEV)].cpu().numpy(), want_rows)}
+
+
+def _completion(rec, parity):
+    """The ALS update of CP completion on the CP-ALS workload of mttkrp_mode ((1e6, 1e6, 100), nnz 1e8, f32), R = 16
+    and 32, modes 0 and 2, the mode stream cached; and on K9's config (1e4, 1e4, 1e3, nnz 1e7, R = 32) next to the
+    composed route: mttkrp_mode with Kronecker-squared factors for the (rows, R^2) Grams, mttkrp_mode for b, and a
+    batched dense solve."""
+    sys.path.insert(0, os.path.join(ROOT, "tests"))
+    out = {}
+    card = _card()
+    reg = 1.0
+    shape = (1_000_000, 1_000_000, 100)
+    X = rand_coo(shape, 100_000_000, 91, torch.float32)
+    for R in (16, 32):
+        g = torch.Generator(device=DEV).manual_seed(92 + R)
+        U = [torch.randn((s, R), generator=g, device=DEV, dtype=torch.float32) for s in shape]
+        for mode in (0, 2):
+            name = f"cp_completion_mode order-3 (1e6,1e6,100) nnz 1e8 R={R} mode {mode} f32"
+            models = _completion_models(X, mode, R)
+            r = rec(name, lambda: sp.cp_completion_mode(X, U, mode, reg), X.nnz, "Gnnz_s", models["bytes"]["total"])
+            r.update({"card": card, **models})
+            if parity:
+                got = sp.cp_completion_mode(X, U, mode, reg)
+                r["parity"] = _completion_parity(X, U, mode, R, reg, got, 8 if mode == 0 else 2, 93)
+                del got
+            out[name] = r
+            print(name, r, flush=True)
+        del U
+    del X
+    torch.cuda.empty_cache()
+
+    I_, K_, L_, R = 10_000, 10_000, 1_000, 32
+    X = rand_coo((I_, K_, L_), 10_000_000, 31, torch.float32)
+    g = torch.Generator(device=DEV).manual_seed(94)
+    U = [torch.randn((s, R), generator=g, device=DEV, dtype=torch.float32) for s in X.shape]
+    sp.mttkrp_mode(X, U, 0)  # the mode stream, cached
+    name = "cp_completion_mode K9 config (1e4,1e4,1e3) nnz 1e7 R=32 mode 0 f32"
+    torch.cuda.synchronize()
+    torch.cuda.reset_peak_memory_stats(DEV)
+    base = torch.cuda.memory_allocated(DEV)
+    r = rec(name, lambda: sp.cp_completion_mode(X, U, 0, reg), X.nnz, "Gnnz_s")
+    ns = R * (R + 1) // 2 + R
+    r.update({"card": card, "peak_extra_bytes_torch": int(torch.cuda.max_memory_allocated(DEV) - base),
+              "crossing_scratch_bytes": 2 * (-(-X.nnz // 512)) * ((ns + 3) // 4 * 4) * 4,
+              **_completion_models(X, 0, R)})
+    fused = sp.cp_completion_mode(X, U, 0, reg)
+    out[name] = r
+
+    coords, _ = X._dev()
+    P = sp.COO(coords, torch.ones(X.nnz, device=DEV), shape=X.shape, has_duplicates=False, sorted=True)
+    sp.mttkrp_mode(P, U, 0)  # X's pattern with ones, its mode stream cached too
+
+    def unfused():
+        Uk = [u[:, :, None] * u[:, None, :] for u in U]
+        Gf = sp.mttkrp_mode(P, [None] + [u.reshape(u.shape[0], R * R) for u in Uk[1:]], 0).reshape(-1, R, R)
+        bf = sp.mttkrp_mode(X, U, 0)
+        return torch.linalg.solve(Gf + reg * torch.eye(R, device=DEV), bf)
+
+    torch.cuda.synchronize()
+    torch.cuda.reset_peak_memory_stats(DEV)
+    base = torch.cuda.memory_allocated(DEV)
+    name_u = "unfused: mttkrp_mode with Kronecker-squared factors + mttkrp_mode + torch.linalg.solve, same config"
+    ru = rec(name_u, unfused, X.nnz, "Gnnz_s")
+    ru.update({"card": card, "peak_extra_bytes_torch": int(torch.cuda.max_memory_allocated(DEV) - base)})
+    x_u = unfused()
+    ru["max_rel_diff_vs_fused"] = float(((x_u.double() - fused.double()).abs().amax(1)
+                                         / fused.double().abs().amax(1).clamp_min(1e-30)).max())
+    out[name_u] = ru
+    del X, P, U, fused, x_u
     torch.cuda.empty_cache()
     return out
 
