@@ -188,16 +188,16 @@ def _tensor_and_factors(name, X, factors, mode, one_rank):
     return N, mode, factors, T, ranks
 
 
-def _mode_product(X, factors, mode, T, W, kernel, rank_arg):
-    """The dense (X.shape[mode], W) result of mttkrp_mode / ttmc_mode after their checks: zeros when nothing is
-    stored, else `kernel` (Kn.mttkrp_mode or Kn.ttmc_mode, given `rank_arg`) over the cached mode stream."""
+def _mode_product(X, factors, mode, T, W, empty, kernel, *args):
+    """The dense (X.shape[mode], W) result of mttkrp_mode / ttmc_mode / cp_completion_mode after their checks: `empty`
+    when nothing is stored, else `kernel(coords, vals, factors, mode, rows, *args)` over the cached mode stream."""
     N, rows = X.ndim, X.shape[mode]
     if X.nnz == 0 or rows == 0 or W == 0:
-        out = Kn.full(rows * W, 0, T).reshape(rows, W)
+        out = Kn.full(rows * W, empty, T).reshape(rows, W)
     else:
         coords, vals = _mode_stream(X, mode)
         fac = [None if m == mode else _dense_dev(factors[m], T) for m in range(N)]
-        out = kernel(coords, Kn.cast(vals, T), fac, mode, rows, rank_arg)
+        out = kernel(coords, Kn.cast(vals, T), fac, mode, rows, *args)
     return _return_dense(out, [f for f in factors if f is not None])
 
 
@@ -222,7 +222,7 @@ def mttkrp_mode(X, factors, mode):
     """
     N, mode, factors, T, ranks = _tensor_and_factors("mttkrp_mode", X, factors, mode, True)
     R = max(ranks)  # the one R of the other factors (ranks[mode] is 0)
-    return _mode_product(X, factors, mode, T, R, Kn.mttkrp_mode, R)
+    return _mode_product(X, factors, mode, T, R, 0, Kn.mttkrp_mode, R)
 
 
 def ttmc_mode(X, factors, mode):
@@ -255,7 +255,7 @@ def ttmc_mode(X, factors, mode):
     if W > Kn.ttmc_mode_max_width():
         raise ValueError(f"ttmc_mode: {W} output columns (the product of the other modes' ranks) exceed the limit of "
                          f"{Kn.ttmc_mode_max_width()}")
-    return _mode_product(X, factors, mode, T, W, Kn.ttmc_mode, ranks)
+    return _mode_product(X, factors, mode, T, W, 0, Kn.ttmc_mode, ranks)
 
 
 def _gcxs_coords(X, limit):
@@ -369,14 +369,7 @@ def cp_completion_mode(X, factors, mode, reg):
         raise ValueError(f"cp_completion_mode: `reg` must be finite and >= 0 in {T}, got {reg!r}")
     if R > Kn.cp_completion_max_rank():
         raise ValueError(f"cp_completion_mode: R = {R} exceeds the limit of {Kn.cp_completion_max_rank()}")
-    rows = X.shape[mode]
-    if X.nnz == 0 or rows == 0 or R == 0:
-        out = Kn.full(rows * R, 0 if reg_t > 0 else np.nan, T).reshape(rows, R)
-    else:
-        coords, vals = _mode_stream(X, mode)
-        fac = [None if m == mode else _dense_dev(factors[m], T) for m in range(N)]
-        out = Kn.cp_completion_mode(coords, Kn.cast(vals, T), fac, mode, rows, R, float(reg_t))
-    return _return_dense(out, [f for f in factors if f is not None])
+    return _mode_product(X, factors, mode, T, R, 0 if reg_t > 0 else np.nan, Kn.cp_completion_mode, R, float(reg_t))
 
 
 # Fibers with more entries than this get whole CTAs in b2s_ttm_mode (a module value so that tests can move it).

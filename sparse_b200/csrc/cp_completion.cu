@@ -15,22 +15,17 @@
 // A row that starts and ends inside the chunk is solved there: its A = G + reg I and b go to shared memory and the
 // CTA factorises A (right-looking, the columns' elements in parallel) and runs the two substitutions.  The first and
 // the last row of a chunk may continue into the neighbouring chunk: their accumulators go to two scratch slots per
-// chunk (K10's scheme), and a second kernel adds each crossing row's slots in chunk order and solves it.  Rows without
-// entries are filled beforehand with the solution of reg I x = 0: +0 for reg > 0, NaN for reg = 0.  No atomics: the
-// result is the order of include/sparse_b200.h, whatever the grid, and the vector and scalar gathers give the same
-// bits.
+// chunk (K10's scheme, from tensor_modes.cuh), and a second kernel adds each crossing row's slots in chunk order and
+// solves it.  Rows without entries are filled beforehand with the solution of reg I x = 0: +0 for reg > 0, NaN for
+// reg = 0.  No atomics: the result is the order of include/sparse_b200.h, whatever the grid, and the vector and scalar
+// gathers give the same bits.
 #include "tensor_modes.cuh"
 
 namespace b2s {
 
-constexpr int64_t kChunk = B2S_MTTKRP_CHUNK;
-constexpr int kMaxOther = 7;  // order <= 8
 constexpr int kThreads = 256;
 constexpr int kBatch = 32;  // entries gathered into shared memory at a time
 constexpr int kMaxRank = B2S_CP_COMPLETION_MAX_RANK;
-
-template <typename I>
-using OtherModes = ModeArrays<I, kMaxOther>;
 
 __device__ __forceinline__ float sub_rn(float a, float b) { return __fsub_rn(a, b); }
 __device__ __forceinline__ double sub_rn(double a, double b) { return __dsub_rn(a, b); }
@@ -162,12 +157,7 @@ cp_completion_kernel(const OtherModes<I> om, const int n_other, const I *__restr
     Smem<T, I> sm(smem_raw, R);
     const int tid = threadIdx.x;
     const int ng = R * (R + 1) / 2, ns = ng + R, hw = 2 * R + 1;
-    const int64_t chunk = blockIdx.x;
-    const int64_t base = chunk * kChunk;
-    const int64_t end = base + kChunk < nnz ? base + kChunk : nnz;
-    const int64_t row_first = (int64_t)rowc[base], row_last = (int64_t)rowc[end - 1];
-    const bool head_cross = chunk > 0 && (int64_t)rowc[base - 1] == row_first;
-    const bool tail_cross = end < nnz && (int64_t)rowc[end] == row_last;
+    const ChunkSpan sp(rowc, nnz, blockIdx.x);
     const uint64_t pol = policy_evict_last();
 
     build_table(sm.tab, R);
@@ -181,15 +171,11 @@ cp_completion_kernel(const OtherModes<I> om, const int n_other, const I *__restr
         tb[k] = t < ns ? sm.tab[t] : 0;
         acc[k] = T(0);
     }
-    int64_t cur = row_first;
+    int64_t cur = sp.row_first;
 
-    // a complete row is solved here; the first row goes to slot 0 when it crosses either boundary, the last row to
-    // slot 1 when it continues into the next chunk (CTA-uniform: every thread sees the same rows)
+    // a complete row is solved here, a crossing one goes to its piece row (CTA-uniform)
     auto flush = [&](int64_t r) {
-        T *dst = nullptr;
-        if (r == row_first && (head_cross || (r == row_last && tail_cross))) dst = pieces + (2 * chunk) * ldp;
-        else if (r == row_last && tail_cross) dst = pieces + (2 * chunk + 1) * ldp;
-        if (dst) {
+        if (T *dst = sp.dest(pieces, ldp, r, (T *)nullptr, 0)) {  // nullptr: solved here
 #pragma unroll
             for (int k = 0; k < KS; ++k)
                 if (tid + k * kThreads < ns) dst[tid + k * kThreads] = acc[k];
@@ -201,8 +187,8 @@ cp_completion_kernel(const OtherModes<I> om, const int n_other, const I *__restr
     };
 
     const int npk = R / VEC;  // packs per factor row
-    for (int64_t b0 = base; b0 < end; b0 += kBatch) {
-        const int n = end - b0 < kBatch ? (int)(end - b0) : kBatch;
+    for (int64_t b0 = sp.base; b0 < sp.end; b0 += kBatch) {
+        const int n = sp.end - b0 < kBatch ? (int)(sp.end - b0) : kBatch;
         if (tid < n) {
             sm.row[tid] = (int64_t)ldg_stream(rowc + b0 + tid);
 #pragma unroll
@@ -251,8 +237,7 @@ cp_completion_kernel(const OtherModes<I> om, const int n_other, const I *__restr
     flush(cur);
 }
 
-// One CTA per chunk boundary b: the row that crosses b and no earlier boundary adds its slots, chunk b-1's first,
-// then the head slots of chunks b .. last (found by bisection), as mttkrp_combine_kernel does; then it is solved.
+// One CTA per chunk boundary b: the row that b owns (crossing_row) adds its NS slots into A and b, then it is solved
 template <typename T, typename I>
 __global__ void __launch_bounds__(kThreads, 1)
 cp_completion_combine_kernel(const I *__restrict__ rowc, const int64_t nnz, const int R, const T reg,
@@ -260,30 +245,20 @@ cp_completion_combine_kernel(const I *__restrict__ rowc, const int64_t nnz, cons
     extern __shared__ __align__(16) unsigned char smem_raw[];
     Smem<T, I> sm(smem_raw, R);
     const int64_t b = (int64_t)blockIdx.x + 1;
-    const int64_t nchunks = (nnz + kChunk - 1) / kChunk;
-    const int64_t p = b * kChunk;
-    const I r = rowc[p];
-    if (rowc[p - 1] != r) return;                    // no row crosses b
-    if (b > 1 && rowc[p - kChunk - 1] == r) return;  // the row crosses b-1 too: that boundary owns it
-    int64_t lo = b, hi = nchunks - 1;
-    while (lo < hi) {
-        const int64_t mid = (lo + hi + 1) >> 1;
-        if (rowc[mid * kChunk] == r) lo = mid;
-        else hi = mid - 1;
-    }
-    const int64_t slot = rowc[p - kChunk] == r ? 0 : 1;
+    int64_t row, first, last;
+    if (!crossing_row(rowc, nnz, b, row, first, last)) return;
     const int ng = R * (R + 1) / 2, ns = ng + R;
     build_table(sm.tab, R);
     __syncthreads();
     for (int t = threadIdx.x; t < ns; t += kThreads) {
         T acc = T(0);
-        acc = add_rn(acc, pieces[(2 * (b - 1) + slot) * ldp + t]);
-        for (int64_t c = b; c <= lo; ++c) acc = add_rn(acc, pieces[(2 * c) * ldp + t]);
+        acc = add_rn(acc, pieces[first * ldp + t]);
+        for (int64_t c = b; c <= last; ++c) acc = add_rn(acc, pieces[(2 * c) * ldp + t]);
         const int l = sm.tab[t] & 0xff, h = sm.tab[t] >> 8;
         if (t < ng) sm.A[h * (R + 1) + l] = l == h ? add_rn(acc, reg) : acc;
         else sm.b[l - R] = acc;
     }
-    solve_row<T>(sm.A, sm.b, sm.y, R, out + (int64_t)r * ldo);
+    solve_row<T>(sm.A, sm.b, sm.y, R, out + row * ldo);
 }
 
 // every row of `out` (rows x R, stride ldo) = v
@@ -349,32 +324,21 @@ static int cp_completion_impl(int order, int mode, int64_t nnz, int64_t rows, in
         ++n_other;
     }
     const I *rowc = (const I *)coords[mode];
-    const int64_t ns = (int64_t)R * (R + 1) / 2 + R;
-    const int64_t ldp = (ns + 3) & ~(int64_t)3;
     const int64_t nchunks = (nnz + kChunk - 1) / kChunk;
     B2S_REQUIRE(nchunks <= INT32_MAX, B2S_ERR_INVALID, "cp_completion_mode: nnz %lld exceeds one grid",
                 (long long)nnz);
-    T *pieces = nullptr;
-    int rc = scratch_alloc((void **)&pieces, (size_t)(2 * nchunks * ldp) * sizeof(T), s);
-    if (rc) return rc;
     const size_t shm = Smem<T, I>::bytes(R);
-    rc = aligned ? dispatch_ks<T, I, VEC>(om, n_other, rowc, vals, nnz, R, reg, out, ldo, pieces, ldp, shm, s)
-                 : dispatch_ks<T, I, 1>(om, n_other, rowc, vals, nnz, R, reg, out, ldo, pieces, ldp, shm, s);
-    cudaError_t e = cudaGetLastError();
-    if (rc == B2S_OK) count_launch();
-    if (rc == B2S_OK && e == cudaSuccess && nchunks > 1) {
+    auto main = [&](T *pieces, int64_t ldp) {
+        return aligned ? dispatch_ks<T, I, VEC>(om, n_other, rowc, vals, nnz, R, reg, out, ldo, pieces, ldp, shm, s)
+                       : dispatch_ks<T, I, 1>(om, n_other, rowc, vals, nnz, R, reg, out, ldo, pieces, ldp, shm, s);
+    };
+    auto combine = [&](T *pieces, int64_t ldp, int64_t) -> int {
         auto kern = cp_completion_combine_kernel<T, I>;
-        if (shm > 48 * 1024) e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)shm);
-        if (e == cudaSuccess) {
-            kern<<<(unsigned)(nchunks - 1), kThreads, shm, s>>>(rowc, nnz, R, reg, pieces, ldp, out, ldo);
-            e = cudaGetLastError();
-            count_launch();
-        }
-    }
-    const int frc = scratch_free(pieces, s);  // stream-ordered: released after the kernels that use it
-    if (rc) return rc;
-    B2S_REQUIRE(e == cudaSuccess, B2S_ERR_CUDA, "cp_completion_mode: kernel launch failed: %s", cudaGetErrorString(e));
-    return frc;
+        if (shm > 48 * 1024) B2S_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)shm));
+        kern<<<(unsigned)(nchunks - 1), kThreads, shm, s>>>(rowc, nnz, R, reg, pieces, ldp, out, ldo);
+        return B2S_OK;
+    };
+    return chunked_launches<T>("cp_completion_mode", nnz, (int64_t)R * (R + 1) / 2 + R, s, main, combine);
 }
 
 }  // namespace b2s

@@ -21,21 +21,15 @@
 //
 // A row that starts and ends inside a chunk is written straight to `out`.  The first and the last row of a chunk may
 // continue into the neighbouring chunk: their partials go to a scratch array (two slots per chunk), and a second
-// kernel adds each crossing row's partials in chunk order.  Rows without entries are zeroed by the chunk that follows
-// them in the stream (the last chunk zeroes the rows after it).  No atomics: the result is the order of
-// include/sparse_b200.h, independent of grid size and scheduling, and the vector and scalar forms are bit-identical.
+// kernel adds each crossing row's partials in chunk order (the chunk scheme of tensor_modes.cuh, shared with K15).
+// Rows without entries are zeroed by the chunk that follows them in the stream (the last chunk zeroes the rows after
+// it).  No atomics: the result is the order of include/sparse_b200.h, independent of grid size and scheduling, and
+// the vector and scalar forms are bit-identical.
 #include <type_traits>
 
 #include "tensor_modes.cuh"
 
 namespace b2s {
-
-constexpr int64_t kChunk = B2S_MTTKRP_CHUNK;
-constexpr int kMaxOther = 7;  // order <= 8
-
-// the gathered other modes, in ascending mode order (K10: all of them; K12: every one but the last)
-template <typename I>
-using OtherModes = ModeArrays<I, kMaxOther>;
 
 // K12: ranks of the leading other modes, ascending
 struct TtmcRanks {
@@ -89,37 +83,27 @@ __device__ __forceinline__ void mode_stream_walk(const OtherModes<I> &om, const 
     using Row = std::conditional_t<KRON, I, int64_t>;  // the type of a shuffled row index (K10 widens it once)
     constexpr unsigned FULL = 0xffffffffu;
 
-    int64_t base = 0, end = 0, row_first = 0, row_last = 0;
-    bool head_cross = false, tail_cross = false;
+    ChunkSpan sp(chunk);  // lanes past the last chunk walk an empty span, but still join the shuffles
     if (chunk < nchunks) {
-        base = chunk * kChunk;
-        end = base + kChunk < nnz ? base + kChunk : nnz;
-        row_first = (int64_t)rowc[base];
-        row_last = (int64_t)rowc[end - 1];
-        const int64_t prev = chunk > 0 ? (int64_t)rowc[base - 1] : -1;
-        head_cross = prev == row_first;
-        tail_cross = end < nnz && (int64_t)rowc[end] == row_last;
+        sp = ChunkSpan(rowc, nnz, chunk);
         if (col_ok) {
-            m_zero_rows<T, VEC>(out, ldo, prev + 1, row_first, col0);
-            if (end == nnz) m_zero_rows<T, VEC>(out, ldo, row_last + 1, rows, col0);
+            m_zero_rows<T, VEC>(out, ldo, sp.prev + 1, sp.row_first, col0);
+            if (sp.end == nnz) m_zero_rows<T, VEC>(out, ldo, sp.row_last + 1, rows, col0);
         }
     }
+    int64_t base = sp.base;
+    const int64_t end = sp.end;
     const uint64_t pol = policy_evict_last();
 
     T acc[VEC];
 #pragma unroll
     for (int k = 0; k < VEC; ++k) acc[k] = T(0);
-    int64_t cur = row_first;
+    int64_t cur = sp.row_first;
 
-    // the first row of the chunk goes to slot 0 when it crosses either boundary, the last row to slot 1 when it
-    // continues into the next chunk; every other row is complete here
+    // a row complete in the chunk goes to `out`, a crossing one to its piece row
     auto flush = [&](int64_t r) {
         if (!col_ok) return;
-        T *dst;
-        if (r == row_first && (head_cross || (r == row_last && tail_cross))) dst = pieces + (2 * chunk) * ldp + col0;
-        else if (r == row_last && tail_cross) dst = pieces + (2 * chunk + 1) * ldp + col0;
-        else dst = out + r * ldo + col0;
-        m_store<T, VEC>(dst, acc);
+        m_store<T, VEC>(sp.dest(pieces + col0, ldp, r, out + col0, ldo), acc);
     };
 
     auto any = [&](bool p) -> bool {
@@ -280,8 +264,7 @@ ttmc_mode_kernel(const OtherModes<I> lead, const TtmcRanks rk, const int n_lead,
                                             ldp);
 }
 
-// One warp per chunk boundary b: the row that crosses b and no earlier boundary adds its partials, chunk b-1's piece
-// first, then the head pieces of chunks b .. last (found by bisection over the chunks' first entries).
+// One warp per chunk boundary b, one column per lane: the row that b owns (crossing_row) adds its pieces into `out`
 template <typename T, typename I>
 __global__ void __launch_bounds__(256)
 mttkrp_combine_kernel(const I *__restrict__ rowc, const int64_t nnz, const int64_t R, const T *__restrict__ pieces,
@@ -290,22 +273,13 @@ mttkrp_combine_kernel(const I *__restrict__ rowc, const int64_t nnz, const int64
     const int64_t nchunks = (nnz + kChunk - 1) / kChunk;
     const int64_t col = (int64_t)blockIdx.y * 32 + (threadIdx.x & 31);
     if (b >= nchunks || col >= R) return;
-    const int64_t p = b * kChunk;
-    const I r = rowc[p];
-    if (rowc[p - 1] != r) return;                  // no row crosses b
-    if (b > 1 && rowc[p - kChunk - 1] == r) return;  // the row crosses b-1 too: that boundary owns it
-    int64_t lo = b, hi = nchunks - 1;
-    while (lo < hi) {
-        const int64_t mid = (lo + hi + 1) >> 1;
-        if (rowc[mid * kChunk] == r) lo = mid;
-        else hi = mid - 1;
-    }
-    const int64_t slot = rowc[p - kChunk] == r ? 0 : 1;
+    int64_t row, first, last;
+    if (!crossing_row(rowc, nnz, b, row, first, last)) return;
     T acc = T(0);
-    acc = add_rn(acc, pieces[(2 * (b - 1) + slot) * ldp + col]);
+    acc = add_rn(acc, pieces[first * ldp + col]);
 #pragma unroll 8
-    for (int64_t c = b; c <= lo; ++c) acc = add_rn(acc, pieces[(2 * c) * ldp + col]);
-    out[(int64_t)r * ldo + col] = acc;
+    for (int64_t c = b; c <= last; ++c) acc = add_rn(acc, pieces[(2 * c) * ldp + col]);
+    out[row * ldo + col] = acc;
 }
 
 // the arguments of one K10 or K12 launch
@@ -409,25 +383,18 @@ static int mode_stream_impl(const char *op, int order, int mode, int64_t nnz, in
     a.W = W;
     a.out = (T *)out;
     a.ldo = ldo;
-    a.ldp = (W + 3) & ~(int64_t)3;  // 16-byte aligned piece rows for both dtypes
-    const int64_t nchunks = (nnz + kChunk - 1) / kChunk;
-    int rc = scratch_alloc((void **)&a.pieces, (size_t)(2 * nchunks * a.ldp) * sizeof(T), s);
-    if (rc) return rc;
-    if (kron) rc = aligned ? dispatch_ttmc<T, I, VEC>(a, s) : dispatch_ttmc<T, I, 1>(a, s);
-    else rc = aligned ? dispatch_mode<T, I, VEC>(a, s) : dispatch_mode<T, I, 1>(a, s);
-    cudaError_t e = cudaGetLastError();
-    if (rc == B2S_OK) count_launch();
-    if (rc == B2S_OK && e == cudaSuccess && nchunks > 1) {
-        const int64_t warps = nchunks - 1;
-        dim3 grid((unsigned)((warps + 7) / 8), (unsigned)((W + 31) / 32));
-        mttkrp_combine_kernel<T, I><<<grid, 256, 0, s>>>(a.rowc, nnz, W, a.pieces, a.ldp, a.out, ldo);
-        e = cudaGetLastError();
-        count_launch();
-    }
-    const int frc = scratch_free(a.pieces, s);  // stream-ordered: released after the kernels that use it
-    if (rc) return rc;
-    B2S_REQUIRE(e == cudaSuccess, B2S_ERR_CUDA, "%s: kernel launch failed: %s", op, cudaGetErrorString(e));
-    return frc;
+    auto main = [&](T *pieces, int64_t ldp) {
+        a.pieces = pieces;
+        a.ldp = ldp;
+        if (kron) return aligned ? dispatch_ttmc<T, I, VEC>(a, s) : dispatch_ttmc<T, I, 1>(a, s);
+        return aligned ? dispatch_mode<T, I, VEC>(a, s) : dispatch_mode<T, I, 1>(a, s);
+    };
+    auto combine = [&](T *pieces, int64_t ldp, int64_t nchunks) -> int {
+        dim3 grid((unsigned)((nchunks - 1 + 7) / 8), (unsigned)((W + 31) / 32));  // a warp per chunk boundary
+        mttkrp_combine_kernel<T, I><<<grid, 256, 0, s>>>(a.rowc, nnz, W, pieces, ldp, a.out, ldo);
+        return B2S_OK;
+    };
+    return chunked_launches<T>(op, nnz, W, s, main, combine);
 }
 
 // what b2s_mttkrp_mode and b2s_ttmc_mode do after their own checks

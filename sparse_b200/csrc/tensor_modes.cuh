@@ -1,10 +1,14 @@
-// tensor_modes.cuh -- what the sparse-tensor kernels K10 / K12 (mttkrp.cu) and K13 (tttp.cu) share: the per-mode
-// pointer arrays, the factor-row pack and its load, and the argument checks and dtype x index-width dispatch of their
-// C entry points.
+// tensor_modes.cuh -- what the sparse-tensor kernels K10 / K12 (mttkrp.cu), K13 (tttp.cu) and K15 (cp_completion.cu)
+// share: the per-mode pointer arrays, the factor-row pack and its load, the argument checks and dtype x index-width
+// dispatch of their C entry points, and the mode-stream chunk scheme of K10, K12 and K15 (one definition, so that
+// K15's b_i stays mttkrp_mode's row bit for bit).
 #pragma once
 #include "common.cuh"
 
 namespace b2s {
+
+constexpr int64_t kChunk = B2S_MTTKRP_CHUNK;
+constexpr int kMaxOther = 7;  // order <= 8
 
 // coordinate array, factor and factor row stride of up to N modes, passed to a kernel by value
 template <typename I, int N>
@@ -13,6 +17,84 @@ struct ModeArrays {
     const void *fac[N];
     int64_t ld[N];
 };
+
+// the gathered other modes of a mode-stream kernel, in ascending mode order
+template <typename I>
+using OtherModes = ModeArrays<I, kMaxOther>;
+
+// Chunk `chunk` of a mode stream (empty for ChunkSpan(c)): its entries base .. end - 1, the row before it (-1 for chunk
+// 0), its first and last row, and whether they continue into the previous / next chunk.
+struct ChunkSpan {
+    int64_t base = 0, end = 0, row_first = 0, row_last = 0, prev = -1, chunk;
+    bool head_cross = false, tail_cross = false;
+
+    __device__ __forceinline__ explicit ChunkSpan(const int64_t c) : chunk(c) {}
+    template <typename I>
+    __device__ __forceinline__ ChunkSpan(const I *rowc, const int64_t nnz, const int64_t c) : chunk(c) {
+        base = c * kChunk;
+        end = base + kChunk < nnz ? base + kChunk : nnz;
+        row_first = (int64_t)rowc[base];
+        row_last = (int64_t)rowc[end - 1];
+        if (c > 0) {
+            prev = (int64_t)rowc[base - 1];
+            head_cross = prev == row_first;
+        }
+        tail_cross = end < nnz && (int64_t)rowc[end] == row_last;
+    }
+
+    // where row r's sums go: piece row 2 chunk (the first row, crossing either boundary) or 2 chunk + 1 (the last row,
+    // continuing into the next chunk) of `pieces`, else row r of `out`, as it is complete in this chunk
+    template <typename T>
+    __device__ __forceinline__ T *dest(T *pieces, const int64_t ldp, const int64_t r, T *out, const int64_t ldo) const {
+        if (r == row_first && (head_cross || (r == row_last && tail_cross))) return pieces + (2 * chunk) * ldp;
+        if (r == row_last && tail_cross) return pieces + (2 * chunk + 1) * ldp;
+        return out + r * ldo;
+    }
+};
+
+// False when no row crosses chunk boundary b >= 1, or when it crosses b-1 too (b-1 owns it).  Else b owns `row`, which
+// adds piece row `first` (chunk b-1's), then the head pieces 2c of chunks c = b .. `last` (found by bisection).
+template <typename I>
+__device__ __forceinline__ bool crossing_row(const I *__restrict__ rowc, const int64_t nnz, const int64_t b,
+                                             int64_t &row, int64_t &first, int64_t &last) {
+    const int64_t p = b * kChunk;
+    const I r = rowc[p];
+    if (rowc[p - 1] != r) return false;                    // no row crosses b
+    if (b > 1 && rowc[p - kChunk - 1] == r) return false;  // the row crosses b-1 too: that boundary owns it
+    int64_t hi = (nnz + kChunk - 1) / kChunk - 1;
+    for (last = b; last < hi;) {
+        const int64_t mid = (last + hi + 1) >> 1;
+        if (rowc[mid * kChunk] == r) last = mid;
+        else hi = mid - 1;
+    }
+    row = (int64_t)r;
+    first = 2 * (b - 1) + (rowc[p - kChunk] == r ? 0 : 1);
+    return true;
+}
+
+// 2 piece rows per chunk, `width` rounded up to 4 (16-byte aligned rows), main(pieces, ldp), combine(pieces, ldp,
+// nchunks) when there is more than one chunk, then the stream-ordered free; each callable launches one kernel
+template <typename T, typename Main, typename Combine>
+int chunked_launches(const char *op, const int64_t nnz, const int64_t width, cudaStream_t s, Main &&main,
+                     Combine &&combine) {
+    const int64_t nchunks = (nnz + kChunk - 1) / kChunk;
+    const int64_t ldp = (width + 3) & ~(int64_t)3;
+    T *pieces = nullptr;
+    int rc = scratch_alloc((void **)&pieces, (size_t)(2 * nchunks * ldp) * sizeof(T), s);
+    if (rc) return rc;
+    rc = main(pieces, ldp);
+    cudaError_t e = cudaGetLastError();
+    if (rc == B2S_OK) count_launch();
+    if (rc == B2S_OK && e == cudaSuccess && nchunks > 1) {
+        rc = combine(pieces, ldp, nchunks);
+        e = cudaGetLastError();
+        if (rc == B2S_OK) count_launch();
+    }
+    const int frc = scratch_free(pieces, s);  // stream-ordered: released after the kernels that use it
+    if (rc) return rc;
+    B2S_REQUIRE(e == cudaSuccess, B2S_ERR_CUDA, "%s: kernel launch failed: %s", op, cudaGetErrorString(e));
+    return frc;
+}
 
 template <typename T, int VEC>
 struct alignas(sizeof(T) * VEC) MPack {
