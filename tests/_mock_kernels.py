@@ -473,6 +473,10 @@ def host_narrow(src, dst):
     return dst
 
 
+# ---- K10-K15: the sparse-tensor ops; K11: masked SpGEMM (stand-ins in their own modules) --------------------------
+from _mock_masked import keys_member, masked_spgemm, masked_spgemm_set_stage, masked_spgemm_sorted  # noqa: E402,F401
+from _mock_tensor import cp_completion_mode, mttkrp_mode, ttm_mode, ttm_mode_long_flags, ttmc_mode, tttp  # noqa: E402,F401
+
 _NAMES = [k for k, v in list(globals().items()) if callable(v) and not k.startswith("_") and hasattr(Kn, k)
           and k not in ("n", "T", "bits_ne", "install", "uninstall")]
 

@@ -1,7 +1,7 @@
 """NumPy stand-in for sparse_b200._kernels.masked_spgemm and its helpers -- TEST INFRASTRUCTURE ONLY.
 
-tests/test_masked_matmul.py puts these in place of the real wrappers for the mock backend (the rest of the kernel layer
-is replaced by _mock_kernels.install()), so the host-side logic of masked_matmul runs without a GPU.  masked_spgemm
+_mock_kernels.install() puts these in place of the real wrappers along with the rest of the kernel layer, so the
+host-side logic of masked_matmul runs without a GPU.  masked_spgemm
 restates the order of b2s_masked_spgemm (include/sparse_b200.h) entry by entry; `order_contract` is the same
 restatement on plain NumPy CSR arrays, shared with the GPU tests and the benchmark's sampled-row check.
 """
@@ -76,8 +76,3 @@ def masked_spgemm_sorted(a_indptr, a_cols, M, bt_indptr, bt_cols, N) -> bool:
 
 def keys_member(query, keys):
     return torch.from_numpy(np.isin(_np(query), _np(keys)).astype(np.uint8))
-
-
-def install(monkeypatch, kernels):
-    for name in ("masked_spgemm", "masked_spgemm_set_stage", "masked_spgemm_sorted", "keys_member"):
-        monkeypatch.setattr(kernels, name, globals()[name])

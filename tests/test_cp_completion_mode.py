@@ -2,47 +2,21 @@
 
 Parity with a float64 NumPy solve of (H_i^T H_i + reg I) x = H_i^T v_i and with the reference's unfused Gram and
 right-hand-side expressions (golden fixture), bit equality with a CPU restatement of the fixed order of operations
-(tests/_completion_order.py) at chunk edges, on both gather paths, with both index widths and special values, the
-identities with mttkrp_mode, edge cases, the mode-stream cache, determinism, errors and ALS convergence.  Every body
-runs on the NumPy mock without a GPU and on the CUDA kernels with `-m gpu`."""
+(tests/_tensor_order.py) at chunk edges, on both gather paths and with special values, the identities with
+mttkrp_mode, edge cases, errors of `reg` and the rank limit, and ALS convergence.  The mode-stream cache, determinism,
+both index widths, factor layouts and the argument errors shared with the other sparse-tensor ops are in
+tests/test_tensor_ops_contract.py.  Every body runs on the NumPy mock without a GPU and on the CUDA kernels with
+`-m gpu`."""
 import numpy as np
 import pytest
 
-import _completion_order as CO
+import _tensor_order as TO
 from _api import dec, sp  # noqa: F401
 from _golden import load
-from test_mttkrp_mode import LAYOUTS, chunk_structured, rand_tensor
-from test_ttm_mode import SHAPES
+from _tensor_cases import LAYOUTS, SHAPES, chunk, chunk_structured, dev, edge_rows, host, rand_tensor
 
 TOL = {"float32": 2e-3, "float64": 1e-9}
-same_bits = CO.same_bits
-
-
-@pytest.fixture(autouse=True)
-def _mock_stand_in(request, monkeypatch):
-    """On the mock backend, the NumPy stand-ins of the K10, K13 and K15 wrappers join the mocked kernel layer."""
-    if "sp" in request.fixturenames:
-        backend = request.getfixturevalue("sp")
-        if backend._device._TEST_CPU:
-            import _mock_completion
-            import _mock_mttkrp
-            import _mock_tttp
-
-            monkeypatch.setattr(backend._kernels, "cp_completion_mode", _mock_completion.cp_completion_mode)
-            monkeypatch.setattr(backend._kernels, "mttkrp_mode", _mock_mttkrp.mttkrp_mode)
-            monkeypatch.setattr(backend._kernels, "tttp", _mock_tttp.tttp)
-
-
-def chunk(sp):
-    return sp._kernels.mttkrp_mode_chunk()
-
-
-def dev(sp, a):
-    return sp._device.upload(np.ascontiguousarray(a))
-
-
-def host(x):
-    return x.detach().cpu().numpy() if hasattr(x, "detach") else np.asarray(x)
+same_bits = TO.same_bits
 
 
 def stored(X):
@@ -73,8 +47,8 @@ def lstsq_ref(X, U, mode, reg, rows=None):
 def order_ref(sp, X, U, mode, dtype, regs):
     """The restatement's result for each reg in `regs` (the sums once, a solve per reg)."""
     coords, vals = stored(X)
-    Gu, b = CO.systems(coords, vals, U, mode, X.shape[mode], chunk(sp), dtype)
-    return [CO.solve(Gu, b, reg, dtype) for reg in regs]
+    Gu, b = TO.systems(coords, vals, U, mode, X.shape[mode], chunk(sp), dtype)
+    return [TO.solve(Gu, b, reg, dtype) for reg in regs]
 
 
 def close(got, want, dtype):
@@ -121,26 +95,6 @@ def test_golden_parity(sp, c):
     close(got, want, c["dtype"])
 
 
-def edge_rows(sp, rng, dtype, R):
-    """Order-3 tensor whose mode-0 rows have 511, 512 and 513 entries around the chunk edges, short rows between them,
-    two empty rows, stored -0.0, +-inf and NaN values in a few rows."""
-    ch = chunk(sp)
-    lengths = [3, ch - 1, ch, 0, ch + 1, 7, 1, ch - 3, 0, 2 * ch, 40]
-    J, K = 40, 60
-    coords, vals = [], []
-    for i, L in enumerate(lengths):
-        lin = np.sort(rng.choice(J * K, size=L, replace=False))
-        coords.append(np.stack([np.full(L, i), lin // K, lin % K]))
-        vals.append(rng.standard_normal(L))
-    coords = np.concatenate(coords, axis=1).astype(np.int64)
-    vals = np.concatenate(vals).astype(dtype)
-    vals[rng.choice(len(vals), 25, replace=False)] = -0.0
-    vals[[2, 100]] = [np.inf, np.nan]  # row 0 becomes non-finite, row 1 NaN
-    X = sp.COO(coords, vals, shape=(len(lengths), J, K), has_duplicates=False, sorted=True)
-    U = [rng.standard_normal((s, R)).astype(dtype) for s in X.shape]
-    return X, U
-
-
 @pytest.mark.parametrize("R", [1, 5, 8, 32])
 @pytest.mark.parametrize("dtype", ["float32", "float64"])
 def test_exact_order(sp, dtype, R):
@@ -183,7 +137,7 @@ def test_rhs_is_mttkrp_mode_and_fully_observed_is_cp_als(sp, dtype):
     U = [rng.standard_normal((s, R)).astype(dtype) for s in shape]
     for mode in range(3):
         # the restatement's right-hand side is mttkrp_mode bit for bit (step 3 of the order)
-        _, b = CO.systems(coords, dense.reshape(-1), U, mode, shape[mode], chunk(sp), dtype)
+        _, b = TO.systems(coords, dense.reshape(-1), U, mode, shape[mode], chunk(sp), dtype)
         assert same_bits(b, sp.mttkrp_mode(X, U, mode))
         # fully observed: the CP-ALS update mttkrp_mode @ inv(hadamard of U_m^T U_m + reg I)
         V = np.ones((R, R))
@@ -248,68 +202,10 @@ def test_edge_cases(sp):
     assert same_bits(got, sp.cp_completion_mode(X, U, -2, 0.5))
 
 
-def test_cache_is_shared_with_mttkrp_mode(sp, monkeypatch):
-    sorts = []
-    real = sp._kernels.sort_keys
-
-    def counting(*a, **k):
-        sorts.append(1)
-        return real(*a, **k)
-
-    monkeypatch.setattr(sp._kernels, "sort_keys", counting)
-    rng = np.random.default_rng(9)
-    X = rand_tensor(sp, rng, (30, 20, 10), 1500, "float64", signed=True)
-    U = [rng.standard_normal((s, 6)) for s in X.shape]
-    for mode in (0, 1, 2):
-        sp.mttkrp_mode(X, U, mode)
-    n = len(sorts)
-    assert n == 2
-    for mode in (0, 1, 2):
-        first = sp.cp_completion_mode(X, U, mode, 0.5)
-        assert same_bits(sp.cp_completion_mode(X, U, mode, 0.5), first)
-    assert len(sorts) == n
-
-
-@pytest.mark.parametrize("dtype", ["float32", "float64"])
-def test_bit_identical_across_calls_locations_and_index_widths(sp, dtype, monkeypatch):
-    rng = np.random.default_rng(10)
-    X = rand_tensor(sp, rng, (70, 60, 8), 9000, dtype, signed=True)
-    U = [rng.standard_normal((s, 12)).astype(dtype) for s in X.shape]
-    Ud = [dev(sp, u) for u in U]
-    for mode in range(3):
-        first = sp.cp_completion_mode(X, U, mode, 0.5)
-        assert same_bits(sp.cp_completion_mode(X, U, mode, 0.5), first)
-        assert same_bits(sp.cp_completion_mode(X.copy(), U, mode, 0.5), first)
-        assert same_bits(host(sp.cp_completion_mode(X, Ud, mode, 0.5)), first)
-        G = X.asformat("gcxs", compressed_axes=(1,))
-        assert same_bits(sp.cp_completion_mode(G, U, mode, 0.5), first)
-        monkeypatch.setattr(sp._fused, "_FORCE_WIDE_INDEX", True)
-        assert same_bits(sp.cp_completion_mode(X, U, mode, 0.5), first)
-        monkeypatch.setattr(sp._fused, "_FORCE_WIDE_INDEX", False)
-    assert all(c.element_size() == 8 for c in X._mode_streams[(1, False)][0])
-    assert all(c.element_size() == 4 for c in X._mode_streams[(1, True)][0])
-
-
 def test_errors(sp, monkeypatch):
     rng = np.random.default_rng(11)
     X = rand_tensor(sp, rng, (5, 6, 7), 40, "float64")
     U = [rng.random((s, 3)) for s in X.shape]
-    with pytest.raises(TypeError):
-        sp.cp_completion_mode(X.todense(), U, 0, 1.0)
-    with pytest.raises(ValueError):
-        sp.cp_completion_mode(rand_tensor(sp, rng, (9,), 4, "float64"), [rng.random((9, 2))], 0, 1.0)
-    with pytest.raises(ValueError, match="zero fill"):
-        sp.cp_completion_mode(sp.COO(X.coords, X.data, shape=X.shape, fill_value=1.0), U, 0, 1.0)
-    for bad in (3, -4):
-        with pytest.raises(np.exceptions.AxisError):
-            sp.cp_completion_mode(X, U, bad, 1.0)
-    with pytest.raises(ValueError):
-        sp.cp_completion_mode(X, U[:2], 0, 1.0)
-    with pytest.raises(ValueError):
-        sp.cp_completion_mode(X, [U[0], rng.random((6, 4)), U[2]], 0, 1.0)
-    with pytest.raises(TypeError, match="outside the CUDA dtype matrix"):
-        Xi = sp.COO(X.coords, np.arange(1, X.nnz + 1), shape=X.shape)
-        sp.cp_completion_mode(Xi, [np.ones((s, 3), np.int64) for s in X.shape], 0, 1.0)
     for bad in (np.nan, np.inf, -np.inf, -1e-3):
         with pytest.raises(ValueError, match="reg"):
             sp.cp_completion_mode(X, U, 0, bad)
@@ -412,13 +308,14 @@ def test_als_completion_large_f32():
     for lo, hi in zip(bounds[0], bounds[1]):
         c = [x[lo:hi].long().cpu().numpy() for x in sc]
         v = sv[lo:hi].cpu().numpy()
-        h, p = CO.khatri_rao(v, [Uh[0][c[0]], Uh[2][c[2]]], np.float32)
-        gu, bb = CO.row_system(h, p, int(lo), 512, np.float32)
+        gathered = [Uh[0][c[0]], Uh[2][c[2]]]
+        h, p = TO.products(None, gathered, np.float32), TO.products(v, gathered, np.float32)
+        gu, bb = TO.row_system(h, p, int(lo), 512, np.float32)
         Gu.append(gu)
         b.append(bb)
         H = Uh[0][c[0]].astype(np.float64) * Uh[2][c[2]].astype(np.float64)
         ref = np.linalg.solve(H.T @ H + np.float64(np.float32(reg)) * np.eye(R), H.T @ v.astype(np.float64))
         np.testing.assert_allclose(got[int(c[1][0])].cpu().numpy(), ref, rtol=1e-2, atol=1e-2 * np.abs(ref).max())
-    want_rows = CO.solve(np.array(Gu), np.array(b), np.float32(reg), np.float32)
+    want_rows = TO.solve(np.array(Gu), np.array(b), np.float32(reg), np.float32)
     assert same_bits(got[torch.from_numpy(rows).to(devc)].cpu().numpy(), want_rows)
 

@@ -17,17 +17,6 @@ from _golden import load
 LAYOUTS = [("coo", None), ("gcxs", (0,)), ("gcxs", (1,))]
 
 
-@pytest.fixture(autouse=True)
-def _mock_stand_in(request, monkeypatch):
-    """On the mock backend, the NumPy stand-ins of the K11 wrappers join the mocked kernel layer."""
-    if "sp" in request.fixturenames:
-        backend = request.getfixturevalue("sp")
-        if backend._device._TEST_CPU:
-            import _mock_masked
-
-            _mock_masked.install(monkeypatch, backend._kernels)
-
-
 def fmt(x, layout):
     kind, ca = LAYOUTS[layout] if isinstance(layout, int) else layout
     return x if kind == "coo" else x.asformat("gcxs", compressed_axes=ca)

@@ -3,39 +3,22 @@ COO result.
 
 Bit identity with ``moveaxis(tensordot(X, U, axes=([mode], [0]), return_type=COO), -1, mode)`` and with the dense
 tensordot at the stored positions, golden parity with the reference's own tensordot (tests/golden/ttm_mode_api.npz),
-shapes far beyond tensordot's size limit against a CPU restatement of the order (tests/_ttm_order.py), the kernel's
-layouts (fiber lengths, group sizes, both end modes, the scalar column path, GCXS layouts), determinism and the
-cached fiber stream, edge cases and errors.  Every body runs on the NumPy mock without a GPU and on the CUDA kernels
-with `-m gpu`."""
+shapes far beyond tensordot's size limit against a CPU restatement of the order (tests/_tensor_order.py), the kernel's
+layouts (fiber lengths, group sizes, both end modes, the scalar column path, GCXS layouts), the cached fiber stream,
+edge cases and errors of U.  Determinism across calls, U's location and layout, both index widths and the argument
+errors shared with the other sparse-tensor ops are in tests/test_tensor_ops_contract.py.  Every body runs on the NumPy
+mock without a GPU and on the CUDA kernels with `-m gpu`."""
 import itertools
 
 import numpy as np
 import pytest
 
-import _ttm_order as TO
+import _tensor_order as TO
 from _api import dec, sp  # noqa: F401
 from _golden import load
-from test_mttkrp_mode import rand_tensor
-from test_ttmc_mode import SHAPES as _SHAPES
+from _tensor_cases import SHAPES, dev, rand_tensor
 
-SHAPES = {**_SHAPES, 7: (3, 2, 3, 2, 2, 3, 2)}  # every order 2..8
 same_bits = TO.same_bits
-
-
-@pytest.fixture(autouse=True)
-def _mock_stand_in(request, monkeypatch):
-    """On the mock backend, the NumPy stand-in of the K14 wrapper joins the mocked kernel layer."""
-    if "sp" in request.fixturenames:
-        backend = request.getfixturevalue("sp")
-        if backend._device._TEST_CPU:
-            import _mock_ttm
-
-            monkeypatch.setattr(backend._kernels, "ttm_mode", _mock_ttm.ttm_mode)
-            monkeypatch.setattr(backend._kernels, "ttm_mode_long_flags", _mock_ttm.ttm_mode_long_flags)
-
-
-def dev(sp, a):
-    return sp._device.upload(np.ascontiguousarray(a))
 
 
 def unfused(sp, X, U, mode, **kw):
@@ -246,24 +229,6 @@ def test_gcxs_layouts(sp):
                 assert_same(sp.ttm_mode(G, U[:, 0], mode), sp.ttm_mode(X, U[:, 0], mode))
 
 
-@pytest.mark.parametrize("dtype", ["float32", "float64"])
-def test_deterministic_locations_and_index_widths(sp, dtype, monkeypatch):
-    rng = np.random.default_rng(23)
-    X = rand_tensor(sp, rng, (40, 30, 20), 6000, dtype, signed=True)
-    for mode in range(3):
-        U = rng.standard_normal((X.shape[mode], 12)).astype(dtype)
-        first = sp.ttm_mode(X, U, mode)
-        for other in (sp.ttm_mode(X, U, mode), sp.ttm_mode(X, dev(sp, U), mode)):
-            assert_same(other, first)
-        monkeypatch.setattr(sp._fused, "_FORCE_WIDE_INDEX", True)
-        wide = sp.ttm_mode(X, U, mode)
-        monkeypatch.setattr(sp._fused, "_FORCE_WIDE_INDEX", False)
-        assert_same(wide, first)
-        narrow, wide_s = X._mode_streams[("fiber", mode, True)], X._mode_streams[("fiber", mode, False)]
-        assert all(x.element_size() == 4 for x in (narrow[0], *narrow[2:5]))
-        assert all(x.element_size() == 8 for x in (wide_s[0], *wide_s[2:5]))
-
-
 def test_second_call_does_not_sort(sp, monkeypatch):
     rng = np.random.default_rng(24)
     X = rand_tensor(sp, rng, (25, 18, 9), 1200, "float64", signed=True)
@@ -334,28 +299,12 @@ def test_edge_cases(sp):
 def test_errors(sp):
     rng = np.random.default_rng(26)
     X = rand_tensor(sp, rng, (5, 6, 7), 40, "float64")
-    U = rng.random((6, 3))
-    with pytest.raises(TypeError):
-        sp.ttm_mode(X.todense(), U, 1)
-    with pytest.raises(ValueError):
-        sp.ttm_mode(rand_tensor(sp, rng, (9,), 4, "float64"), rng.random((9, 2)), 0)
-    nine = sp.COO(np.zeros((9, 1), np.int64), np.ones(1), shape=(2,) * 9)
-    with pytest.raises(ValueError):
-        sp.ttm_mode(nine, np.ones((2, 2)), 0)
-    with pytest.raises(ValueError, match="zero fill"):
-        sp.ttm_mode(sp.COO(X.coords, X.data, shape=X.shape, fill_value=1.0), U, 1)
-    for mode in (3, -4):
-        with pytest.raises(np.exceptions.AxisError):
-            sp.ttm_mode(X, U, mode)
     with pytest.raises(ValueError, match="shape mismatch"):
         sp.ttm_mode(X, rng.random((5, 3)), 1)
     with pytest.raises(ValueError, match="shape mismatch"):
         sp.ttm_mode(X, rng.random(7), 1)
     with pytest.raises(ValueError, match="shape mismatch"):
         sp.ttm_mode(X, rng.random((6, 3, 2)), 1)
-    with pytest.raises(TypeError, match="outside the CUDA dtype matrix"):
-        Xi = sp.COO(X.coords, np.arange(1, X.nnz + 1), shape=X.shape)
-        sp.ttm_mode(Xi, np.ones((6, 3), np.int64), 1)
     with pytest.raises(TypeError, match="outside the CUDA dtype matrix"):
         sp.ttm_mode(X, np.ones((6, 3), np.complex128), 1)
     big = sp.COO(np.zeros((3, 1), np.int64), np.ones(1), shape=(2**31, 2**31, 1))

@@ -1,64 +1,28 @@
 """ttmc_mode(X, factors, mode): mode-n TTMc (tensor times matrix chain) of sparse tensors of order 2..8.
 
 Parity with float64 dense einsum and with the reference's unfused broadcast expression (golden fixture), bit equality
-with a CPU restatement of the fixed order of operations (tests/_ttmc_order.py) on both column paths, the diagonal
-identity with mttkrp_mode, determinism, the mode-stream cache shared with mttkrp_mode, the int64 index path, edge cases,
-errors, and a small HOOI that reconstructs a tensor of exact multilinear rank.  Every body runs on the NumPy mock
-without a GPU and on the CUDA kernels with `-m gpu`."""
-import string
-
+with a CPU restatement of the fixed order of operations (tests/_tensor_order.py) on both column paths, the diagonal
+identity with mttkrp_mode, edge cases, the width limit, and a small HOOI that reconstructs a tensor of exact multilinear
+rank.  Determinism, the mode-stream cache shared with mttkrp_mode, the int64 index path, factor layouts and the shared
+argument errors are in tests/test_tensor_ops_contract.py.  Every body runs on the NumPy mock without a GPU and on the
+CUDA kernels with `-m gpu`."""
 import numpy as np
 import pytest
 
-import _ttmc_order as TO
+import _tensor_order as TO
 from _api import dec, sp  # noqa: F401
 from _golden import load
-from test_mttkrp_mode import LAYOUTS, chunk_structured, rand_tensor
+from _tensor_cases import (LAYOUTS, SHAPES, chunk, chunk_structured, dev, full_size_tensor, host, layout_id,
+                           plant_specials, rand_tensor, ttmc_einsum as einsum_ref)
 
 TOL = {"float32": 2e-5, "float64": 1e-12}
 same_bits = TO.same_bits
-
-
-@pytest.fixture(autouse=True)
-def _mock_stand_in(request, monkeypatch):
-    """On the mock backend, the NumPy stand-ins of the K10 and K12 wrappers join the mocked kernel layer."""
-    if "sp" in request.fixturenames:
-        backend = request.getfixturevalue("sp")
-        if backend._device._TEST_CPU:
-            import _mock_mttkrp
-            import _mock_ttmc
-
-            monkeypatch.setattr(backend._kernels, "mttkrp_mode", _mock_mttkrp.mttkrp_mode)
-            monkeypatch.setattr(backend._kernels, "ttmc_mode", _mock_ttmc.ttmc_mode)
-
-
-def chunk(sp):
-    return sp._kernels.mttkrp_mode_chunk()
-
-
-def dev(sp, a):
-    return sp._device.upload(np.asarray(a))
-
-
-def host(x):
-    return x.detach().cpu().numpy() if hasattr(x, "detach") else np.asarray(x)
 
 
 def factors(rng, shape, ranks, dtype, signed=False):
     if signed:
         return [rng.standard_normal((s, r)).astype(dtype) for s, r in zip(shape, ranks)]
     return [rng.random((s, r)).astype(dtype) + np.asarray(0.05, dtype) for s, r in zip(shape, ranks)]
-
-
-def einsum_ref(X, U, mode):
-    """float64 einsum with output subscripts "i" + "abc...", flattened to (I_mode, W)."""
-    N = X.ndim
-    lo, hi = string.ascii_lowercase[:N], string.ascii_uppercase[:N]
-    others = [m for m in range(N) if m != mode]
-    terms = [lo] + [lo[m] + hi[m] for m in others]
-    ops = [X.todense().astype(np.float64)] + [np.asarray(U[m], np.float64) for m in others]
-    out = np.einsum(",".join(terms) + "->" + lo[mode] + "".join(hi[m] for m in others), *ops)
-    return out.reshape(X.shape[mode], -1)
 
 
 def order_ref(sp, X, U, mode, dtype):
@@ -70,8 +34,6 @@ def width(U, mode):
     return int(np.prod([u.shape[1] for m, u in enumerate(U) if m != mode]))
 
 
-SHAPES = {2: (37, 29), 3: (23, 17, 11), 4: (9, 7, 6, 5), 5: (6, 5, 4, 3, 5), 6: (4, 3, 3, 2, 3, 2),
-          8: (3, 2, 3, 2, 2, 3, 2, 2)}
 # per order: unequal ranks (R_last often not a multiple of 16 B / itemsize), and a set whose W spans several column
 # tiles of both paths
 RANKS = {2: [(3, 5), (70, 150)], 3: [(3, 4, 2), (12, 16, 9)], 4: [(2, 3, 5, 4), (4, 6, 8, 5)],
@@ -81,8 +43,8 @@ RANKS = {2: [(3, 5), (70, 150)], 3: [(3, 4, 2), (12, 16, 9)], 4: [(2, 3, 5, 4), 
 
 @pytest.mark.parametrize("rset", [0, 1], ids=["small", "wide"])
 @pytest.mark.parametrize("dtype", ["float32", "float64"])
-@pytest.mark.parametrize("order", sorted(SHAPES))
-@pytest.mark.parametrize("layout", range(len(LAYOUTS)), ids=lambda i: LAYOUTS[i][0] + str(LAYOUTS[i][1] or ""))
+@pytest.mark.parametrize("order", [2, 3, 4, 5, 6, 8])
+@pytest.mark.parametrize("layout", range(len(LAYOUTS)), ids=layout_id)
 def test_fp64_parity_every_mode(sp, order, dtype, rset, layout):
     shape, ranks = SHAPES[order], RANKS[order][rset]
     fmt, ca = LAYOUTS[layout]
@@ -121,12 +83,7 @@ def test_golden_parity(sp, c, fmt):
 
 def special_factors(rng, shape, ranks, dtype):
     """Signed normal factors with +-inf, NaN and -0.0 planted in each."""
-    U = factors(rng, shape, ranks, dtype, signed=True)
-    for u in U:
-        flat = u.reshape(-1)
-        k = min(4, flat.size)
-        flat[rng.choice(flat.size, k, replace=False)] = [np.inf, -np.inf, np.nan, -0.0][:k]
-    return U
+    return plant_specials(rng, factors(rng, shape, ranks, dtype, signed=True))
 
 
 # (ranks, what they exercise): f32 vector packs hold 4 columns and f64 ones 2, so R_last = 8 takes the vector path in
@@ -153,25 +110,17 @@ def test_exact_order_skewed_mode_order4(sp):
 
 @pytest.mark.parametrize("dtype", ["float32", "float64"])
 def test_vector_and_scalar_paths_agree(sp, dtype):
-    """The same values through aligned contiguous factors (vector path), a Fortran-ordered copy, a device column-major
-    view, and a device view one column into a wider buffer (unaligned rows: scalar path)."""
-    import torch
-
+    """The restatement's bits through aligned contiguous factors (vector path where R_last fills whole 16-byte packs)
+    and through device views one column into a wider buffer (unaligned rows: scalar path); a float64 factor promotes
+    the result.  Fortran-ordered, transposed and mixed host / device factors are in test_tensor_ops_contract.py."""
     rng = np.random.default_rng(31)
     X = rand_tensor(sp, rng, (40, 30, 20), 2500, dtype, signed=True)
     U = special_factors(rng, X.shape, (5, 6, 8), dtype)
-    want = [order_ref(sp, X, U, m, dtype) for m in range(3)]
-    fortran = [np.asfortranarray(u) for u in U]
-    transposed = [dev(sp, u.T.copy()).T for u in U]
     wide = [dev(sp, np.concatenate([np.zeros((u.shape[0], 1), dtype), u], axis=1))[:, 1:] for u in U]
-    mixed = [U[0], dev(sp, U[1]), U[2]]
     for m in range(3):
-        assert same_bits(sp.ttmc_mode(X, U, m), want[m])
-        assert same_bits(sp.ttmc_mode(X, fortran, m), want[m])
-        for variant in (transposed, wide, mixed):
-            got = sp.ttmc_mode(X, variant, m)
-            assert isinstance(got, torch.Tensor)
-            assert same_bits(host(got), want[m])
+        want = order_ref(sp, X, U, m, dtype)
+        assert same_bits(sp.ttmc_mode(X, U, m), want), m
+        assert same_bits(host(sp.ttmc_mode(X, wide, m)), want), m
     U64 = [U[0].astype(np.float64), U[1], U[2]]
     got = sp.ttmc_mode(X, U64, 1)
     assert got.dtype == np.float64
@@ -196,64 +145,6 @@ def test_diagonal_equals_mttkrp_mode(sp, order, dtype, R):
         assert same_bits(diagonal(t, shape[mode], R, order - 1), k), mode
         if order == 2:
             assert same_bits(t, k)
-
-
-@pytest.mark.parametrize("dtype", ["float32", "float64"])
-def test_determinism(sp, dtype):
-    rng = np.random.default_rng(11)
-    X = rand_tensor(sp, rng, (70, 60, 8), 9000, dtype, signed=True)
-    U = factors(rng, X.shape, (6, 5, 12), dtype, signed=True)
-    Ud = [dev(sp, u) for u in U]
-    for mode in range(3):
-        first = sp.ttmc_mode(X, U, mode)
-        for _ in range(3):
-            assert same_bits(sp.ttmc_mode(X, U, mode), first)
-        assert same_bits(sp.ttmc_mode(X.copy(), U, mode), first)  # the copy builds its stream again
-        assert same_bits(host(sp.ttmc_mode(X, Ud, mode)), first)
-
-
-def test_cache_is_shared_with_mttkrp_mode(sp, monkeypatch):
-    Kn = sp._kernels
-    calls = []
-    real = Kn.sort_keys
-
-    def counting(*a, **k):
-        calls.append(1)
-        return real(*a, **k)
-
-    monkeypatch.setattr(Kn, "sort_keys", counting)
-    rng = np.random.default_rng(3)
-    X = rand_tensor(sp, rng, (30, 20, 10), 1500, "float64", signed=True)
-    U = factors(rng, X.shape, (4, 4, 4), "float64", signed=True)
-    for mode in (1, 2):
-        calls.clear()
-        sp.mttkrp_mode(X, U, mode)
-        assert len(calls) == 1, mode
-        first = sp.ttmc_mode(X, U, mode)
-        sp.ttmc_mode(X, U, mode)
-        assert len(calls) == 1, mode  # the stream mttkrp_mode built is reused
-        fresh = X.copy()
-        assert fresh._mode_streams is None
-        assert same_bits(sp.ttmc_mode(fresh, U, mode), first)
-    calls.clear()
-    Y = X.copy()
-    sp.ttmc_mode(Y, U, 2)
-    sp.mttkrp_mode(Y, U, 2)  # and the other way round
-    assert len(calls) == 1
-    np.multiply(Y, 2, out=Y)  # new contents drop the cache
-    assert same_bits(sp.ttmc_mode(Y, U, 2), 2 * sp.ttmc_mode(X, U, 2))
-
-
-def test_int64_index_path(sp, monkeypatch):
-    rng = np.random.default_rng(19)
-    X = rand_tensor(sp, rng, (50, 40, 9), 4000, "float32", signed=True)
-    U = factors(rng, X.shape, (6, 4, 16), "float32", signed=True)
-    narrow = [sp.ttmc_mode(X, U, m) for m in range(3)]
-    monkeypatch.setattr(sp._fused, "_FORCE_WIDE_INDEX", True)
-    for m in range(3):
-        assert same_bits(sp.ttmc_mode(X, U, m), narrow[m])
-    assert all(c.element_size() == 8 for c in X._mode_streams[(1, False)][0])
-    assert all(c.element_size() == 4 for c in X._mode_streams[(1, True)][0])
 
 
 def test_edge_cases(sp):
@@ -281,28 +172,6 @@ def test_edge_cases(sp):
 def test_errors(sp):
     rng = np.random.default_rng(23)
     X = rand_tensor(sp, rng, (5, 6, 7), 40, "float64")
-    U = [rng.random((s, r)) for s, r in zip(X.shape, (2, 3, 4))]
-    with pytest.raises(TypeError):
-        sp.ttmc_mode(X.todense(), U, 0)
-    with pytest.raises(ValueError):
-        sp.ttmc_mode(rand_tensor(sp, rng, (9,), 4, "float64"), [rng.random((9, 2))], 0)
-    nine = sp.COO(np.zeros((9, 1), np.int64), np.ones(1), shape=(2,) * 9)
-    with pytest.raises(ValueError):
-        sp.ttmc_mode(nine, [np.ones((2, 2))] * 9, 0)
-    with pytest.raises(ValueError, match="zero fill"):
-        sp.ttmc_mode(sp.COO(X.coords, X.data, shape=X.shape, fill_value=1.0), U, 0)
-    for bad in (3, -4):
-        with pytest.raises(np.exceptions.AxisError):
-            sp.ttmc_mode(X, U, bad)
-    with pytest.raises(ValueError):
-        sp.ttmc_mode(X, U[:2], 0)
-    with pytest.raises(ValueError):
-        sp.ttmc_mode(X, [U[0], rng.random((5, 3)), U[2]], 0)
-    with pytest.raises(ValueError):
-        sp.ttmc_mode(X, [U[0], rng.random(6), U[2]], 0)
-    with pytest.raises(TypeError, match="outside the CUDA dtype matrix"):
-        Xi = sp.COO(X.coords, np.arange(1, X.nnz + 1), shape=X.shape)
-        sp.ttmc_mode(Xi, [np.ones((s, 3), np.int64) for s in X.shape], 0)
     limit = sp._kernels.ttmc_mode_max_width()
     assert limit == 65535 * 32
     big = [None, np.ones((6, 1449)), np.ones((7, 1448))]  # W = 2,098,152
@@ -342,15 +211,9 @@ def test_full_size_each_mode():
 
     import sparse_b200 as spm
 
-    devc = torch.device("cuda")
-    shape, nnz, R = (1_000_000, 1_000_000, 100), 100_000_000, 16
-    g = torch.Generator(device=devc).manual_seed(78)
-    lin = torch.unique(torch.randint(0, shape[0] * shape[1] * shape[2], (nnz,), generator=g, device=devc))
-    coords = torch.stack(torch.unravel_index(lin, shape))
-    del lin
-    vals = torch.rand(coords.shape[1], generator=g, device=devc) + 0.1
-    X = spm.COO(coords, vals, shape=shape, has_duplicates=False, sorted=True)
-    U = [torch.rand((s, R), generator=g, device=devc) + 0.05 for s in shape]
+    X, coords, vals, g = full_size_tensor(78)
+    shape, R = X.shape, 16
+    U = [torch.rand((s, R), generator=g, device=coords.device) + 0.05 for s in shape]
     ch = spm._kernels.mttkrp_mode_chunk()
     rng = np.random.default_rng(6)
     for mode in range(3):
@@ -359,17 +222,13 @@ def test_full_size_each_mode():
         assert got.shape == (shape[mode], R * R)
         step = 10_000_000
         for ra in range(R):  # columns ra * R .. ra * R + R - 1
-            want = torch.zeros((shape[mode], R), dtype=torch.float64, device=devc)
+            want = torch.zeros((shape[mode], R), dtype=torch.float64, device=coords.device)
             for s in range(0, coords.shape[1], step):
                 c = coords[:, s:s + step]
                 p = vals[s:s + step].double() * U[a][c[a], ra].double()
                 want.index_add_(0, c[mode], p[:, None] * U[b][c[b]].double())
             assert torch.allclose(got[:, ra * R:(ra + 1) * R].double(), want, rtol=2e-5, atol=0), (mode, ra)
         del want
-        for i in rng.choice(shape[mode], 4, replace=False):
-            sel = torch.nonzero(coords[mode] == int(i)).reshape(-1)  # C order = stream order inside the row
-            start = int((coords[mode] < int(i)).sum())
-            c = coords[:, sel]
-            p = TO.products(vals[sel].cpu().numpy(), [U[m][c[m]].cpu().numpy() for m in (a, b)], np.float32)
-            assert same_bits(got[int(i)].cpu().numpy(), TO.row_result(p, start, ch, np.float32)), (mode, i)
+        rows = rng.choice(shape[mode], 4, replace=False)
+        assert TO.sampled_rows_exact(got, coords, vals, U, mode, rows, ch, kron=True), mode
         del got

@@ -1,68 +1,24 @@
 """tttp(X, factors): a sparse tensor of order 2..8 times a CP model at its stored entries (X * [[U_0, ..., U_{N-1}]]).
 
 Parity with float64 dense `X * einsum(...)` and with the reference's unfused broadcast expression (golden fixture), bit
-equality with a CPU restatement of the fixed order of operations (tests/_tttp_order.py) on both column paths with
-special values, order 2 against sddmm, the result's pattern and format, the absence of sorts, determinism across
-calls, factor locations and index widths, identities with mttkrp_mode, edge cases and errors.  Every body runs on the
-NumPy mock without a GPU and on the CUDA kernels with `-m gpu`."""
+equality with a CPU restatement of the fixed order of operations (tests/_tensor_order.py) on both column paths with
+special values, order 2 against sddmm, the result's pattern and format, the absence of sorts, identities with
+mttkrp_mode, edge cases and the `None` factor.  Determinism across calls, factor locations and layouts, index widths and
+the shared argument errors are in tests/test_tensor_ops_contract.py.  Every body runs on the NumPy mock without a GPU
+and on the CUDA kernels with `-m gpu`."""
 import string
 
 import numpy as np
 import pytest
 
-import _tttp_order as TP
+import _tensor_order as TO
 from _api import dec, sp  # noqa: F401
 from _golden import load
-from test_mttkrp_mode import LAYOUTS, rand_tensor
-from test_ttmc_mode import SHAPES
+from _tensor_cases import (LAYOUTS, SHAPES, dev, entries, full_size_tensor, layout, layout_id, model_dense,
+                           rand_tensor)
 
 TOL = {"float32": 2e-5, "float64": 1e-12}
-same_bits = TP.same_bits
-
-
-@pytest.fixture(autouse=True)
-def _mock_stand_in(request, monkeypatch):
-    """On the mock backend, the NumPy stand-ins of the K10 and K13 wrappers join the mocked kernel layer."""
-    if "sp" in request.fixturenames:
-        backend = request.getfixturevalue("sp")
-        if backend._device._TEST_CPU:
-            import _mock_mttkrp
-            import _mock_tttp
-
-            monkeypatch.setattr(backend._kernels, "mttkrp_mode", _mock_mttkrp.mttkrp_mode)
-            monkeypatch.setattr(backend._kernels, "tttp", _mock_tttp.tttp)
-
-
-def dev(sp, a):
-    return sp._device.upload(np.asarray(a))
-
-
-def layout(X, fmt, ca):
-    if fmt == "coo":
-        return X
-    return X.asformat("gcxs", compressed_axes=(X.ndim - 1,) if ca == "last" else ca)
-
-
-def entries(X):
-    """(coordinates N x nnz, values) of X's entries in its stored order."""
-    if X.format == "coo":
-        return np.asarray(X.coords, np.int64), np.asarray(X.data)
-    ca = list(X.compressed_axes)
-    order = ca + [a for a in range(X.ndim) if a not in ca]
-    rs = [X.shape[a] for a in order]
-    rows = np.repeat(np.arange(len(X.indptr) - 1), np.diff(X.indptr))
-    parts = list(np.unravel_index(rows, rs[:len(ca)])) + list(np.unravel_index(X.indices, rs[len(ca):]))
-    coords = np.zeros((X.ndim, X.nnz), np.int64)
-    for pos, a in enumerate(order):
-        coords[a] = parts[pos]
-    return coords, np.asarray(X.data)
-
-
-def model_dense(U):
-    """float64 CP model [[U_0, ..., U_{N-1}]] as a dense array."""
-    N = len(U)
-    lo = string.ascii_lowercase[:N]
-    return np.einsum(",".join(c + "z" for c in lo) + "->" + lo, *[np.asarray(u, np.float64) for u in U])
+same_bits = TO.same_bits
 
 
 def positive_zero(z):
@@ -71,10 +27,10 @@ def positive_zero(z):
 
 
 def check_exact(sp, got, X, U, dtype):
-    """got holds X's entries, in X's stored order, minus those whose z is bitwise +0, with the bits of _tttp_order."""
+    """got holds X's entries, in X's stored order, minus those whose z is bitwise +0, with the bits of _tensor_order."""
     dtype = np.dtype(dtype)
     coords, vals = entries(X)
-    z = TP.values(coords, vals, U, dtype)
+    z = TO.values(coords, vals, U, dtype)
     keep = ~positive_zero(z)
     assert got.format == X.format and got.shape == X.shape and got.dtype == dtype
     assert same_bits(np.asarray(got.fill_value), np.asarray(dtype.type(0)))
@@ -89,8 +45,8 @@ def check_exact(sp, got, X, U, dtype):
 # R = 1, 3 and 37 take the scalar path in both dtypes; 32 and 300 the vector path (300 is ten f32 or 19 f64 r-tiles)
 @pytest.mark.parametrize("R", [1, 3, 32, 37, 300])
 @pytest.mark.parametrize("dtype", ["float32", "float64"])
-@pytest.mark.parametrize("order", sorted(SHAPES))
-@pytest.mark.parametrize("lay", range(len(LAYOUTS)), ids=lambda i: LAYOUTS[i][0] + str(LAYOUTS[i][1] or ""))
+@pytest.mark.parametrize("order", [2, 3, 4, 5, 6, 8])
+@pytest.mark.parametrize("lay", range(len(LAYOUTS)), ids=layout_id)
 def test_fp64_parity(sp, lay, order, dtype, R):
     shape = SHAPES[order]
     fmt, ca = LAYOUTS[lay]
@@ -156,7 +112,7 @@ def test_exact_order_both_paths(sp, dtype, R):
         Y = layout(X, fmt, ca)
         keep = check_exact(sp, sp.tttp(Y, U), Y, U, dtype)
         _, vals = entries(Y)
-        z = TP.values(entries(Y)[0], vals, U, dtype)
+        z = TO.values(entries(Y)[0], vals, U, dtype)
         assert (~keep).sum() > 0 and np.signbit(z[~keep]).sum() == 0
         assert (np.signbit(z) & (z == 0)).any()  # stored -0.0 results
         assert np.isnan(z).any()
@@ -239,26 +195,6 @@ def test_no_sort(sp, monkeypatch):
 
 
 @pytest.mark.parametrize("dtype", ["float32", "float64"])
-def test_bit_identical_across_calls_locations_and_index_widths(sp, dtype, monkeypatch):
-    rng = np.random.default_rng(14)
-    X = rand_tensor(sp, rng, (70, 60, 8), 9000, dtype, signed=True)
-    U = [rng.standard_normal((s, 24)).astype(dtype) for s in X.shape]
-    Ud = [dev(sp, u) for u in U]
-    for fmt, ca in LAYOUTS:
-        Y = layout(X, fmt, ca)
-        first = sp.tttp(Y, U)
-        for other in (sp.tttp(Y, U), sp.tttp(Y, Ud), sp.tttp(Y, [U[0], Ud[1], U[2]])):
-            assert np.array_equal(entries(other)[0], entries(first)[0])
-            assert same_bits(other.data, first.data)
-        monkeypatch.setattr(sp._fused, "_FORCE_WIDE_INDEX", True)
-        wide = sp.tttp(Y, U)
-        monkeypatch.setattr(sp._fused, "_FORCE_WIDE_INDEX", False)
-        assert same_bits(wide.data, first.data)
-    assert all(c.element_size() == 8 for c in X._mode_streams[(0, False)][0])
-    assert all(c.element_size() == 4 for c in X._mode_streams[(0, True)][0])
-
-
-@pytest.mark.parametrize("dtype", ["float32", "float64"])
 def test_identities_with_mttkrp_mode(sp, dtype):
     rng = np.random.default_rng(15)
     X = rand_tensor(sp, rng, (20, 16, 12, 6), 1500, dtype, signed=True)
@@ -305,37 +241,15 @@ def test_edge_cases(sp):
     for fmt, ca in LAYOUTS:
         got = sp.tttp(layout(one, fmt, ca), U)
         assert got.nnz == 1
-        assert same_bits(got.data, TP.values([[4], [5], [6]], [2.0], U, np.float64))
+        assert same_bits(got.data, TO.values([[4], [5], [6]], [2.0], U, np.float64))
 
 
 def test_errors(sp):
     rng = np.random.default_rng(17)
     X = rand_tensor(sp, rng, (5, 6, 7), 40, "float64")
     U = [rng.random((s, 3)) for s in X.shape]
-    with pytest.raises(TypeError):
-        sp.tttp(X.todense(), U)
-    with pytest.raises(ValueError):
-        sp.tttp(rand_tensor(sp, rng, (9,), 4, "float64"), [rng.random((9, 2))])
-    nine = sp.COO(np.zeros((9, 1), np.int64), np.ones(1), shape=(2,) * 9)
-    with pytest.raises(ValueError):
-        sp.tttp(nine, [np.ones((2, 2))] * 9)
-    with pytest.raises(ValueError, match="zero fill"):
-        sp.tttp(sp.COO(X.coords, X.data, shape=X.shape, fill_value=1.0), U)
-    with pytest.raises(ValueError):
-        sp.tttp(X, U[:2])
-    with pytest.raises(ValueError):
-        sp.tttp(X, U + [U[0]])
-    with pytest.raises(ValueError):
-        sp.tttp(X, [U[0], rng.random((5, 3)), U[2]])
-    with pytest.raises(ValueError):
-        sp.tttp(X, [U[0], rng.random((6, 4)), U[2]])
-    with pytest.raises(ValueError):
-        sp.tttp(X, [U[0], rng.random(6), U[2]])
     with pytest.raises(ValueError, match="None"):
         sp.tttp(X, [None, U[1], U[2]])
-    with pytest.raises(TypeError, match="outside the CUDA dtype matrix"):
-        Xi = sp.COO(X.coords, np.arange(1, X.nnz + 1), shape=X.shape)
-        sp.tttp(Xi, [np.ones((s, 3), np.int64) for s in X.shape])
 
 
 @pytest.mark.gpu
@@ -346,17 +260,9 @@ def test_full_size():
 
     import sparse_b200 as spm
 
-    devc = torch.device("cuda")
-    shape, nnz, R = (1_000_000, 1_000_000, 100), 100_000_000, 32
-    g = torch.Generator(device=devc).manual_seed(79)
-    lin = torch.unique(torch.randint(0, shape[0] * shape[1] * shape[2], (nnz,), generator=g, device=devc))
-    coords = torch.stack(torch.unravel_index(lin, shape))
-    del lin
-    sign = torch.randint(0, 2, (coords.shape[1],), generator=g, device=devc) * 2 - 1
-    vals = (torch.rand(coords.shape[1], generator=g, device=devc) + 0.1) * sign  # no zero value: nothing is pruned
-    del sign
-    X = spm.COO(coords, vals, shape=shape, has_duplicates=False, sorted=True)
-    U = [torch.rand((s, R), generator=g, device=devc) + 0.05 for s in shape]
+    X, coords, vals, g = full_size_tensor(79, signed=True)  # no zero value: nothing is pruned
+    R = 32
+    U = [torch.rand((s, R), generator=g, device=coords.device) + 0.05 for s in X.shape]
     got = spm.tttp(X, U)
     assert got.nnz == coords.shape[1]
     gv = got._data_dev()
@@ -367,7 +273,7 @@ def test_full_size():
         want = vals[s:s + step].double() * m
         assert torch.allclose(gv[s:s + step].double(), want, rtol=2e-5, atol=0), s
     rng = np.random.default_rng(6)
-    pick = torch.from_numpy(np.sort(rng.choice(coords.shape[1], 10_000, replace=False))).to(devc)
+    pick = torch.from_numpy(np.sort(rng.choice(coords.shape[1], 10_000, replace=False))).to(coords.device)
     c = coords[:, pick].cpu().numpy()
-    want = TP.values(c, vals[pick].cpu().numpy(), [u.cpu().numpy() for u in U], np.float32)
+    want = TO.values(c, vals[pick].cpu().numpy(), [u.cpu().numpy() for u in U], np.float32)
     assert same_bits(gv[pick].cpu().numpy(), want)

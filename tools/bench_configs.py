@@ -411,7 +411,7 @@ def _mttkrp_mode_order3(rec, parity):
     """CP-ALS workload: (1e6, 1e6, 100) with 1e8 uniform entries, R = 32, f32, factors on the device.  Modes 0 and 1
     have ~100 entries per slice, mode 2 has 100 slices of ~1e6 entries (the skewed case)."""
     sys.path.insert(0, os.path.join(ROOT, "tests"))
-    import _mttkrp_order as MO
+    import _tensor_order as TO
 
     shape, R = (1_000_000, 1_000_000, 100), 32
     X = rand_coo(shape, 100_000_000, 41, torch.float32)
@@ -446,17 +446,10 @@ def _mttkrp_mode_order3(rec, parity):
             close = bool(torch.allclose(got.double(), want, rtol=2e-5, atol=0))
             del want
             rows = np.random.default_rng(mode).choice(shape[mode], 4, replace=False)
-            exact = True
-            for i in rows:
-                sel = torch.nonzero(coords[mode] == int(i)).reshape(-1)
-                start = int((coords[mode] < int(i)).sum())
-                c = coords[:, sel]
-                p = MO.products(vals[sel].cpu().numpy(), [U[m][c[m]].cpu().numpy() for m in range(N) if m != mode],
-                                np.float32)
-                exact &= MO.same_bits(got[int(i)].cpu().numpy(), MO.row_result(p, start, ch, np.float32))
+            exact = TO.sampled_rows_exact(got, coords, vals, U, mode, rows, ch, kron=False)
             r["parity"] = {"vs": "fp64 device restatement (all rows, rtol 2e-5) + 4 sampled rows bit-compared with "
-                                 "the CPU restatement of the order (tests/_mttkrp_order.py)",
-                           "values_close": close, "sampled_rows_bit_exact": bool(exact)}
+                                 "the CPU restatement of the order (tests/_tensor_order.py)",
+                           "values_close": close, "sampled_rows_bit_exact": exact}
         out[name] = r
     del X, U, coords, vals
     return out
@@ -464,8 +457,8 @@ def _mttkrp_mode_order3(rec, parity):
 
 def _ttmc_parity(X, U, mode, got, ranks, sample_rows, seed):
     """fp64 device restatement of every row (one block of R_last columns per leading digit, entries in blocks of 1e7)
-    and `sample_rows` rows bit-compared with the CPU restatement of the order (tests/_ttmc_order.py)."""
-    import _ttmc_order as TO
+    and `sample_rows` rows bit-compared with the CPU restatement of the order (tests/_tensor_order.py)."""
+    import _tensor_order as TO
 
     coords, vals = X._dev()
     shape, nnz = X.shape, X.nnz
@@ -480,17 +473,11 @@ def _ttmc_parity(X, U, mode, got, ranks, sample_rows, seed):
             want.index_add_(0, c[mode], p[:, None] * U[b][c[b]].double())
         close &= bool(torch.allclose(got[:, ra * Rb:(ra + 1) * Rb].double(), want, rtol=2e-5, atol=0))
         del want
-    exact = True
-    ch = sp._kernels.mttkrp_mode_chunk()
-    for i in np.random.default_rng(seed).choice(shape[mode], sample_rows, replace=False):
-        sel = torch.nonzero(coords[mode] == int(i)).reshape(-1)
-        start = int((coords[mode] < int(i)).sum())
-        c = coords[:, sel]
-        p = TO.products(vals[sel].cpu().numpy(), [U[m][c[m]].cpu().numpy() for m in (a, b)], np.float32)
-        exact &= TO.same_bits(got[int(i)].cpu().numpy(), TO.row_result(p, start, ch, np.float32))
+    rows = np.random.default_rng(seed).choice(shape[mode], sample_rows, replace=False)
+    exact = TO.sampled_rows_exact(got, coords, vals, U, mode, rows, sp._kernels.mttkrp_mode_chunk(), kron=True)
     return {"vs": f"fp64 device restatement (all rows, rtol 2e-5) + {sample_rows} sampled rows bit-compared with the "
-                  "CPU restatement of the order (tests/_ttmc_order.py)",
-            "values_close": close, "sampled_rows_bit_exact": bool(exact)}
+                  "CPU restatement of the order (tests/_tensor_order.py)",
+            "values_close": close, "sampled_rows_bit_exact": exact}
 
 
 def _ttmc_models(X, ranks, mode, vb=4, ib=4):
@@ -593,8 +580,8 @@ def _ttmc(rec, parity):
 
 def _tttp_parity(X, U, got, samples, seed):
     """Every entry against an fp64 device restatement (rtol 2e-5) and `samples` sampled entries bit-compared with the
-    CPU restatement of the order (tests/_tttp_order.py).  X is COO; `got` has X's pattern (nothing pruned)."""
-    import _tttp_order as TP
+    CPU restatement of the order (tests/_tensor_order.py).  X is COO; `got` has X's pattern (nothing pruned)."""
+    import _tensor_order as TO
 
     coords, vals = X._dev()
     gv = got._data_dev()
@@ -608,11 +595,11 @@ def _tttp_parity(X, U, got, samples, seed):
                                      rtol=2e-5, atol=0))
         del m
     pick = torch.from_numpy(np.sort(np.random.default_rng(seed).choice(X.nnz, samples, replace=False))).to(DEV)
-    want = TP.values(coords[:, pick].cpu().numpy(), vals[pick].cpu().numpy(), [u.cpu().numpy() for u in U],
+    want = TO.values(coords[:, pick].cpu().numpy(), vals[pick].cpu().numpy(), [u.cpu().numpy() for u in U],
                      np.float32)
     return {"vs": f"fp64 device restatement (all entries, rtol 2e-5) + {samples} sampled entries bit-compared with the "
-                  "CPU restatement of the order (tests/_tttp_order.py)",
-            "values_close": close, "sampled_entries_bit_exact": TP.same_bits(gv[pick].cpu().numpy(), want)}
+                  "CPU restatement of the order (tests/_tensor_order.py)",
+            "values_close": close, "sampled_entries_bit_exact": TO.same_bits(gv[pick].cpu().numpy(), want)}
 
 
 def _tttp_models(X, R, vb=4, ib=4):
@@ -636,7 +623,7 @@ def _tttp(rec, parity):
     f32, COO and one GCXS layout); at order 2 on C4's shape next to sddmm, alternating; and on K9's config next to the
     unfused einsum("ijk,ir,jr,kr->ijk"), whose nnz * R products are what the fused kernel avoids."""
     sys.path.insert(0, os.path.join(ROOT, "tests"))
-    import _tttp_order as TP
+    import _tensor_order as TO
 
     out = {}
     card = _card()
@@ -660,7 +647,7 @@ def _tttp(rec, parity):
     if parity:
         gc = sp.tttp(G, U).tocoo()
         r["parity"] = {"vs": "the COO result (GCXS result converted to COO)",
-                       "bit_exact": bool(TP.same_bits(gc.data, sp.tttp(X, U).data))}
+                       "bit_exact": bool(TO.same_bits(gc.data, sp.tttp(X, U).data))}
         del gc
     out[name] = r
     del X, G, U
@@ -745,8 +732,8 @@ def _ttm_models(X, nf, R, vb=4, ib=4):
 
 def _ttm_parity(X, U, mode, got, samples, seed):
     """Every value against an fp64 device restatement (per-fiber index_add of v * U[k], rtol 2e-5), and `samples`
-    sampled fibers bit-compared with the CPU restatement of the order (tests/_ttm_order.py)."""
-    import _ttm_order as TO
+    sampled fibers bit-compared with the CPU restatement of the order (tests/_tensor_order.py)."""
+    import _tensor_order as TO
 
     coords, vals = X._dev()
     shape, N = X.shape, X.ndim
@@ -798,7 +785,7 @@ def _ttm_parity(X, U, mode, got, samples, seed):
     exact = bool(np.array_equal(got_c, rc) and TO.same_bits(gv[gsel].cpu().numpy(), rv))
     return {"vs": f"fp64 device restatement (all values, within max(rtol 2e-5, (L + 1) * 2**-24 * sum |v * U|) for a "
                   f"fiber of L entries) + {samples} sampled fibers bit-compared with the CPU restatement of the order "
-                  "(tests/_ttm_order.py)",
+                  "(tests/_tensor_order.py)",
             "values_close": close, "sampled_fibers_bit_exact": exact}
 
 
@@ -849,7 +836,6 @@ def _ttm(rec, parity):
     uniform, one with Zipf fiber lengths up to 1e6 entries -- timed against it alternating, with both calls' peak extra
     device memory."""
     sys.path.insert(0, os.path.join(ROOT, "tests"))
-    import _ttm_order as TO
 
     out = {}
     card = _card()
@@ -937,8 +923,8 @@ def _completion_models(X, mode, R, vb=4, ib=4):
 
 def _completion_parity(X, U, mode, R, reg, got, sample_rows, seed):
     """Every row against an fp64 device solve of (G_i + reg I) x = b_i (G and b summed in fp64), and `sample_rows`
-    rows bit-compared with the CPU restatement of the order (tests/_completion_order.py)."""
-    import _completion_order as CO
+    rows bit-compared with the CPU restatement of the order (tests/_tensor_order.py)."""
+    import _tensor_order as TO
 
     coords, vals = X._dev()
     rows = X.shape[mode]
@@ -968,15 +954,15 @@ def _completion_parity(X, U, mode, R, reg, got, sample_rows, seed):
     Gu, bb = [], []
     for lo, hi in zip(bounds[0], bounds[1]):
         gathered = [U[m][sc[m][lo:hi].long()].cpu().numpy() for m in others]
-        h, p = CO.khatri_rao(sv[lo:hi].cpu().numpy(), gathered, np.float32)
-        gu, bi = CO.row_system(h, p, int(lo), 512, np.float32)
+        h, p = TO.products(None, gathered, np.float32), TO.products(sv[lo:hi].cpu().numpy(), gathered, np.float32)
+        gu, bi = TO.row_system(h, p, int(lo), 512, np.float32)
         Gu.append(gu)
         bb.append(bi)
-    want_rows = CO.solve(np.array(Gu), np.array(bb), np.float32(reg), np.float32)
+    want_rows = TO.solve(np.array(Gu), np.array(bb), np.float32(reg), np.float32)
     return {"vs": f"fp64 device solve of every row (max |x - x64| / max |x64| <= 1e-3) + {sample_rows} sampled rows "
-                  "bit-compared with the CPU restatement of the order (tests/_completion_order.py)",
+                  "bit-compared with the CPU restatement of the order (tests/_tensor_order.py)",
             "values_close": close, "worst_row_rel_err": worst,
-            "sampled_rows_bit_exact": CO.same_bits(got[torch.from_numpy(pick).to(DEV)].cpu().numpy(), want_rows)}
+            "sampled_rows_bit_exact": TO.same_bits(got[torch.from_numpy(pick).to(DEV)].cpu().numpy(), want_rows)}
 
 
 def _completion(rec, parity):
