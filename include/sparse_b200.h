@@ -378,6 +378,39 @@ int b2s_cp_completion_mode(int dtype, int idx_bytes, int order, int mode, int64_
                            const void *const *factors_host, const int64_t *ld_host, void *out_dev, int64_t ldo,
                            void *stream);
 
+/* ---- the ratio MTTKRP Phi of Poisson CP (CP-APR), mode n of a sparse tensor of order 2..8 (K16, cp_apr.cu; no
+ * reference counterpart) --------------------------------------------------------------------------------------------
+ * out[i, r] = sum over stored entries e with i_mode(e) = i of w_e * prod_{m != mode} U_m[i_m(e), r], with
+ * w_e = v_e / max(m_e, eps) and m_e = sum_r prod_m U_m[i_m(e), r] the CP model at e over ALL factors (U_mode, the
+ * factor being updated, included).  Arguments as b2s_mttkrp_mode (the same MODE STREAM S_mode, factors of R columns),
+ * except that every factor is read, and extents_host[m] is the number of rows of factor m (a factor that is not
+ * 16-byte aligned with a row stride that is a multiple of 16 / itemsize, or an R that is not such a multiple, is read
+ * through an aligned copy of its rows); eps is finite and >= 0 in the value type and is cast to it;
+ * R <= B2S_CP_APR_PHI_MAX_RANK.  out is dense (rows x R, row stride ldo), fully written.  Scratch: the aligned
+ * copies, and two slots of R values per chunk for the rows that cross chunks.  No atomics, no stream synchronisation.
+ *
+ * Fixed order of operations (results are reproducible bit for bit, whatever the grid, SM count, index width, stream or
+ * factor layout); every operation is rounded separately, no FMA contraction:
+ *  1. The input is the mode stream S_mode, cut into chunks of B2S_MTTKRP_CHUNK entries, as b2s_mttkrp_mode's steps 1
+ *     and 3.
+ *  2. m_e is b2s_tttp's steps 1-2 over all `order` factors, U_mode at its own position: q_r = ((U_0[i_0, r] *
+ *     U_1[i_1, r]) * U_2[i_2, r]) * ..., ascending over the modes, and m_e = ((+0 + q_0) + q_1) + ..., ascending in r.
+ *     So m_e is b2s_tttp's value at e for the values 1, bit for bit.
+ *  3. d_e = eps if m_e < eps, else m_e (a NaN m_e stays NaN).
+ *  4. w_e = v_e / d_e, correctly rounded.
+ *  5. p_e[r] = ((w_e * U_a[i_a, r]) * U_b[i_b, r]) * ... over the modes a < b < ... other than `mode`: b2s_mttkrp_mode's
+ *     step 2 with v_e replaced by w_e.
+ *  6. Partials per (chunk, row) and row results over the chunks are b2s_mttkrp_mode's steps 4 and 5; a row without
+ *     entries is +0.
+ * So the result is b2s_mttkrp_mode's for the values w_e, bit for bit.
+ */
+#define B2S_CP_APR_PHI_MAX_RANK 64
+int b2s_cp_apr_phi_max_rank(void); /* returns B2S_CP_APR_PHI_MAX_RANK */
+int b2s_cp_apr_phi_mode(int dtype, int idx_bytes, int order, int mode, int64_t nnz, int64_t rows, int64_t R,
+                        double eps, const void *const *coords_host, const void *vals_dev,
+                        const void *const *factors_host, const int64_t *ld_host, const int64_t *extents_host,
+                        void *out_dev, int64_t ldo, void *stream);
+
 /* ---- a sparse tensor of order 2..8 times a CP model at its stored entries (K13, tttp.cu; TTTP, the order-N SDDMM,
  * no reference counterpart) ------------------------------------------------------------------------------------------
  * out_vals[e] = v_e * sum_r U_0[i_0(e), r] * U_1[i_1(e), r] * ... * U_{order-1}[i_{order-1}(e), r] for each of the nnz

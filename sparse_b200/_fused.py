@@ -13,6 +13,9 @@ Kronecker counterpart, the TTMc step of Tucker / HOOI, with the same inputs and 
 evaluates a CP model at X's stored entries (X * [[U_0, ..., U_{N-1}]], the order-N sddmm) and keeps X's pattern.
 ttm_mode(X, U, mode) is the mode-n tensor times matrix (or vector) with a sparse result: tensordot(X, U, axes=([mode],
 [0])) bit for bit, in O(nnz + result) memory instead of a dense intermediate over the other extents.
+cp_completion_mode(X, factors, mode, reg) is the row-wise least-squares ALS update of CP completion, and
+cp_apr_phi_mode(X, factors, mode, eps) the ratio MTTKRP of Poisson CP (CP-APR): mttkrp_mode of X / max(model, eps)
+at X's entries, fused on the same cached mode stream.
 
 masked_matmul(mask, a, b) == mask * (a @ b) at mask's stored positions, for sparse a and b: the masked SpGEMM of
 examples/triangles_example.py (sum(a @ a * a) / 6) and of the GraphBLAS masked mxm.  It never forms the product
@@ -370,6 +373,73 @@ def cp_completion_mode(X, factors, mode, reg):
     if R > Kn.cp_completion_max_rank():
         raise ValueError(f"cp_completion_mode: R = {R} exceeds the limit of {Kn.cp_completion_max_rank()}")
     return _mode_product(X, factors, mode, T, R, 0 if reg_t > 0 else np.nan, Kn.cp_completion_mode, R, float(reg_t))
+
+
+def cp_apr_phi_mode(X, factors, mode, eps=1e-10):
+    """The ratio MTTKRP Phi of Poisson CP (CP-APR, Chi & Kolda 2012): the product of the mode-`mode` matricisation of
+    X / max(model, eps), taken at X's stored entries, with the Khatri-Rao product of every other factor -- the kernel
+    that CP-APR's multiplicative update runs up to l_max times per mode and outer iteration.
+
+        m_e      = sum_r prod_m factors[m][i_m(e), r]             (the CP model at entry e, factors[mode] included)
+        out[i, r] = sum over stored entries e with i_mode(e) = i of  v_e / max(m_e, eps) * prod_{m != mode} factors[m][i_m(e), r]
+
+    `X` is a COO or GCXS of order 2..8 with a zero fill value.  `factors` holds N dense 2-D arrays (NumPy arrays or CUDA
+    tensors, which may be mixed), `factors[m]` of shape (X.shape[m], R) with one R for all; every factor is read,
+    `factors[mode]` (B, the factor being updated, with the weights absorbed) included.  `eps` is a finite real >= 0,
+    cast to the result dtype.  The result is dense, (X.shape[mode], R), of dtype result_type(X.dtype, factor dtypes)
+    (float32 or float64): a NumPy array, or a CUDA tensor when a factor is one.  Rows without entries are +0.  R is at
+    most `_kernels.cp_apr_phi_max_rank()` (64); a larger R raises ValueError before anything is allocated.
+
+    CP-APR expects X >= 0 and nonnegative factors; signs are not checked (that would read the data back from the
+    device), and the formula is computed for any inputs.  One difference from MATLAB's ``max(M, eps)``: a NaN model
+    value stays NaN rather than becoming eps, so that a NaN in the model shows up instead of turning into v / eps.
+
+    The order of operations is fixed (include/sparse_b200.h, b2s_cp_apr_phi_mode), so results are reproducible bit for
+    bit.  m_e is `tttp(P, factors)` at e bit for bit (P: X's pattern with ones), and the result is
+    ``mttkrp_mode(COO(X.coords, w), factors, mode)`` bit for bit, with w_e = v_e / max(m_e, eps) correctly rounded.
+
+    One CP-APR multiplicative-update (MU) sweep over the modes, the factors' columns summing to 1 and the weights lam
+    absorbed into the mode being updated:
+
+        for n in range(X.ndim):
+            B = U[n] * lam
+            for it in range(l_max):                            # inner iterations, typically 10
+                Phi = cp_apr_phi_mode(X, U[:n] + [B] + U[n + 1:], n, eps)
+                if np.abs(np.minimum(B, 1 - Phi)).max() < tol:  # the KKT test
+                    break
+                B = B * Phi                                    # the multiplicative update
+            lam = B.sum(axis=0)                                # column normalisation
+            U[n] = B / lam
+        P = COO(X.coords, np.ones(X.nnz), shape=X.shape)       # X's pattern with ones
+        m = tttp(P, [U[0] * lam] + U[1:]).data                 # the model at X's entries (positive, so all stored)
+        nll = lam.sum() - (X.data * np.log(m)).sum()           # the negative log-likelihood
+
+    Memory: the mode stream of `mode`, cached on `X` and shared with `mttkrp_mode`, `ttmc_mode` and
+    `cp_completion_mode` (not rebuilt); the result, rows * R * itemsize; and, during the call, a scratch array of
+    2 * ceil(nnz / 512) * R' * itemsize bytes (R' = R rounded up to a multiple of 4) for the rows that cross chunks,
+    plus an aligned copy of any factor whose rows are not 16-byte aligned or whose R is not a multiple of
+    16 / itemsize.  No nnz-sized intermediate is formed.
+    """
+    name = "cp_apr_phi_mode"
+    N, _, factors, T, ranks = _tensor_and_factors(name, X, factors, None, True)
+    _, mode = _tensor_and_mode(name, X, mode)
+    R = ranks[0]
+    if isinstance(eps, (bool, np.bool_)) or not isinstance(eps, (int, float, np.integer, np.floating)):
+        raise TypeError(f"{name}: `eps` must be a real number, got {type(eps).__name__}")
+    with np.errstate(over="ignore"):
+        eps_t = T.type(eps)
+    if not np.isfinite(eps_t) or eps_t < 0:
+        raise ValueError(f"{name}: `eps` must be finite and >= 0 in {T}, got {eps!r}")
+    if R > Kn.cp_apr_phi_max_rank():
+        raise ValueError(f"{name}: R = {R} exceeds the limit of {Kn.cp_apr_phi_max_rank()}")
+    rows = X.shape[mode]
+    if X.nnz == 0 or rows == 0 or R == 0:
+        out = Kn.full(rows * R, 0, T).reshape(rows, R)
+    else:
+        coords, vals = _mode_stream(X, mode)
+        fac = [_dense_dev(f, T) for f in factors]
+        out = Kn.cp_apr_phi_mode(coords, Kn.cast(vals, T), fac, mode, rows, R, float(eps_t))
+    return _return_dense(out, factors)
 
 
 # Fibers with more entries than this get whole CTAs in b2s_ttm_mode (a module value so that tests can move it).

@@ -758,6 +758,30 @@ def cp_completion_mode(coords, vals, factors, mode, rows, R, reg):
 
 
 # ------------------------------------------------------------------------------------------------
+# K16 CP-APR ratio MTTKRP
+# ------------------------------------------------------------------------------------------------
+def cp_apr_phi_max_rank() -> int:
+    """Largest R that b2s_cp_apr_phi_mode accepts (B2S_CP_APR_PHI_MAX_RANK)."""
+    return int(_lib.load().b2s_cp_apr_phi_max_rank())
+
+
+def cp_apr_phi_mode(coords, vals, factors, mode, rows, R, eps):
+    """out[i, r] = sum over the stream entries e with coords[mode][e] = i of w_e * prod_{m != mode}
+    factors[m][coords[m][e], r], w_e = vals[e] / max(m_e, eps) with m_e the CP model of every factor at e, in the fixed
+    order of b2s_cp_apr_phi_mode.  `coords` (N index tensors, one width) and `vals` are the mode stream; every factor
+    is read; `eps` is a Python float already rounded to the value type."""
+    N = len(coords)
+    ptrs, fptrs, ld, keep = _factor_args(coords, vals, factors, [R] * N)
+    out = _t().empty((rows, R), dtype=vals.dtype, device=vals.device)
+    rc = _lib.load().b2s_cp_apr_phi_mode(i32(D.dtype_code(D.np_dtype(vals))), i32(_idx_bytes(coords[0])), i32(N),
+                                         i32(mode), i64(vals.shape[0]), i64(rows), i64(R), ctypes.c_double(eps), ptrs,
+                                         vp(D.ptr(vals)), fptrs, ld, _i64arr([int(f.shape[0]) for f in factors]),
+                                         vp(D.ptr(out)), i64(R), _sp())
+    _lib.check(rc, "b2s_cp_apr_phi_mode")
+    return out
+
+
+# ------------------------------------------------------------------------------------------------
 # K14 mode-n TTM
 # ------------------------------------------------------------------------------------------------
 def ttm_mode_long_flags(fptr, long_min):

@@ -264,24 +264,6 @@ ttmc_mode_kernel(const OtherModes<I> lead, const TtmcRanks rk, const int n_lead,
                                             ldp);
 }
 
-// One warp per chunk boundary b, one column per lane: the row that b owns (crossing_row) adds its pieces into `out`
-template <typename T, typename I>
-__global__ void __launch_bounds__(256)
-mttkrp_combine_kernel(const I *__restrict__ rowc, const int64_t nnz, const int64_t R, const T *__restrict__ pieces,
-                      const int64_t ldp, T *__restrict__ out, const int64_t ldo) {
-    const int64_t b = (((int64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5) + 1;
-    const int64_t nchunks = (nnz + kChunk - 1) / kChunk;
-    const int64_t col = (int64_t)blockIdx.y * 32 + (threadIdx.x & 31);
-    if (b >= nchunks || col >= R) return;
-    int64_t row, first, last;
-    if (!crossing_row(rowc, nnz, b, row, first, last)) return;
-    T acc = T(0);
-    acc = add_rn(acc, pieces[first * ldp + col]);
-#pragma unroll 8
-    for (int64_t c = b; c <= last; ++c) acc = add_rn(acc, pieces[(2 * c) * ldp + col]);
-    out[row * ldo + col] = acc;
-}
-
 // the arguments of one K10 or K12 launch
 template <typename T, typename I>
 struct StreamArgs {
@@ -389,10 +371,8 @@ static int mode_stream_impl(const char *op, int order, int mode, int64_t nnz, in
         if (kron) return aligned ? dispatch_ttmc<T, I, VEC>(a, s) : dispatch_ttmc<T, I, 1>(a, s);
         return aligned ? dispatch_mode<T, I, VEC>(a, s) : dispatch_mode<T, I, 1>(a, s);
     };
-    auto combine = [&](T *pieces, int64_t ldp, int64_t nchunks) -> int {
-        dim3 grid((unsigned)((nchunks - 1 + 7) / 8), (unsigned)((W + 31) / 32));  // a warp per chunk boundary
-        mttkrp_combine_kernel<T, I><<<grid, 256, 0, s>>>(a.rowc, nnz, W, pieces, ldp, a.out, ldo);
-        return B2S_OK;
+    auto combine = [&](T *pieces, int64_t ldp, int64_t nchunks) {
+        return launch_mttkrp_combine<T, I>(a.rowc, nnz, W, pieces, ldp, nchunks, a.out, ldo, s);
     };
     return chunked_launches<T>(op, nnz, W, s, main, combine);
 }

@@ -1,11 +1,14 @@
-// tensor_modes.cuh -- what the sparse-tensor kernels K10 / K12 (mttkrp.cu), K13 (tttp.cu) and K15 (cp_completion.cu)
-// share: the per-mode pointer arrays, the factor-row pack and its load, the argument checks and dtype x index-width
-// dispatch of their C entry points, and the mode-stream chunk scheme of K10, K12 and K15 (one definition, so that
-// K15's b_i stays mttkrp_mode's row bit for bit).
+// tensor_modes.cuh -- what the sparse-tensor kernels K10 / K12 (mttkrp.cu), K13 (tttp.cu), K15 (cp_completion.cu) and
+// K16 (cp_apr.cu) share: the per-mode pointer arrays, the factor-row pack and its load, the argument checks and dtype x
+// index-width dispatch of their C entry points, and the mode-stream chunk scheme of K10, K12, K15 and K16 with K10's
+// combine kernel (one definition, so that K15's b_i and K16's sums stay mttkrp_mode's rows bit for bit).
 #pragma once
 #include "common.cuh"
 
 namespace b2s {
+
+__device__ __forceinline__ float div_rn(float a, float b) { return __fdiv_rn(a, b); }
+__device__ __forceinline__ double div_rn(double a, double b) { return __ddiv_rn(a, b); }
 
 constexpr int64_t kChunk = B2S_MTTKRP_CHUNK;
 constexpr int kMaxOther = 7;  // order <= 8
@@ -70,6 +73,34 @@ __device__ __forceinline__ bool crossing_row(const I *__restrict__ rowc, const i
     row = (int64_t)r;
     first = 2 * (b - 1) + (rowc[p - kChunk] == r ? 0 : 1);
     return true;
+}
+
+// K10's combine, also K16's (the sums of both are b2s_mttkrp_mode's steps 4-5): one warp per chunk boundary b, one
+// column per lane; the row that b owns (crossing_row) adds its pieces into `out`
+template <typename T, typename I>
+__global__ void __launch_bounds__(256)
+mttkrp_combine_kernel(const I *__restrict__ rowc, const int64_t nnz, const int64_t R, const T *__restrict__ pieces,
+                      const int64_t ldp, T *__restrict__ out, const int64_t ldo) {
+    const int64_t b = (((int64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5) + 1;
+    const int64_t nchunks = (nnz + kChunk - 1) / kChunk;
+    const int64_t col = (int64_t)blockIdx.y * 32 + (threadIdx.x & 31);
+    if (b >= nchunks || col >= R) return;
+    int64_t row, first, last;
+    if (!crossing_row(rowc, nnz, b, row, first, last)) return;
+    T acc = T(0);
+    acc = add_rn(acc, pieces[first * ldp + col]);
+#pragma unroll 8
+    for (int64_t c = b; c <= last; ++c) acc = add_rn(acc, pieces[(2 * c) * ldp + col]);
+    out[row * ldo + col] = acc;
+}
+
+// the combine launch of R columns over the nchunks - 1 chunk boundaries: a warp per boundary
+template <typename T, typename I>
+int launch_mttkrp_combine(const I *rowc, const int64_t nnz, const int64_t R, const T *pieces, const int64_t ldp,
+                          const int64_t nchunks, T *out, const int64_t ldo, cudaStream_t s) {
+    dim3 grid((unsigned)((nchunks - 1 + 7) / 8), (unsigned)((R + 31) / 32));
+    mttkrp_combine_kernel<T, I><<<grid, 256, 0, s>>>(rowc, nnz, R, pieces, ldp, out, ldo);
+    return B2S_OK;
 }
 
 // 2 piece rows per chunk, `width` rounded up to 4 (16-byte aligned rows), main(pieces, ldp), combine(pieces, ldp,

@@ -5,11 +5,11 @@ Device-resident inputs (generated with seeded torch generators on the GPU), wall
 torch.cuda.synchronize() because the public calls contain their own size-returning syncs.
 Prints one line per config as it runs and the whole result as one JSON line at the end.
 
-    python tools/bench_configs.py [c1 c3 c3big red c4 c5 mttkrp mttkrp_mode masked ttmc tttp ttm completion]
+    python tools/bench_configs.py [c1 c3 c3big red c4 c5 mttkrp mttkrp_mode masked ttmc tttp ttm completion cp_apr]
 
 `masked` (the masked SpGEMM, examples/triangles_example.py), `ttmc` (the Tucker / HOOI step), `tttp` (a CP model at
-a sparse tensor's entries), `ttm` (mode-n tensor times matrix with a sparse result) and `completion` (the ALS update
-of CP tensor completion) run only when named.
+a sparse tensor's entries), `ttm` (mode-n tensor times matrix with a sparse result), `completion` (the ALS update
+of CP tensor completion) and `cp_apr` (the ratio MTTKRP of Poisson CP) run only when named.
 """
 import json
 import os
@@ -288,6 +288,8 @@ def run(which=None, compact=False, parity=True):
         res.update(_ttm(rec, parity))
     if "completion" in which:
         res.update(_completion(rec, parity))
+    if "cp_apr" in which:
+        res.update(_cp_apr(rec, parity))
     torch.cuda.empty_cache()
     return res
 
@@ -1032,6 +1034,152 @@ def _completion(rec, parity):
                                          / fused.double().abs().amax(1).clamp_min(1e-30)).max())
     out[name_u] = ru
     del X, P, U, fused, x_u
+    torch.cuda.empty_cache()
+    return out
+
+
+def _phi_models(X, mode, R, vb=4, ib=4):
+    """Byte model of one cp_apr_phi_mode call (f32, int32 coordinates): the mode stream, one R-column row of every
+    factor per entry counted as if every gather came from HBM, the result, and the crossing rows' scratch written and
+    read."""
+    N, nnz = X.ndim, X.nnz
+    nchunks = -(-nnz // 512)
+    b = {"stream": nnz * (N * ib + vb), "factor_gathers": nnz * N * R * vb, "output": X.shape[mode] * R * vb,
+         "crossing_scratch": 2 * 2 * nchunks * ((R + 3) // 4 * 4) * vb}
+    b["total"] = sum(b.values())
+    return {"bytes": b, "model_ms_bytes_at_3.35TBs": round(b["total"] / 3.35e12 * 1e3, 3)}
+
+
+def _alternate(fns, reps=5, warm=2):
+    """Median ms of each callable, the callables timed in turn within every repetition."""
+    for _ in range(warm):
+        for f in fns.values():
+            f()
+    torch.cuda.synchronize()
+    ts = {k: [] for k in fns}
+    for _ in range(reps):
+        for k, f in fns.items():
+            torch.cuda.synchronize()
+            t0 = time.perf_counter()
+            f()
+            torch.cuda.synchronize()
+            ts[k].append((time.perf_counter() - t0) * 1e3)
+    return {k: round(float(np.median(v)), 4) for k, v in ts.items()}
+
+
+def _phi_parity(X, U, mode, eps, got, sample_rows, seed):
+    """Every row against an fp64 device evaluation, and `sample_rows` rows bit-compared with the CPU restatement of
+    the order (tests/_cp_apr_order.py)."""
+    import _cp_apr_order as CA
+
+    coords, vals = X._dev()
+    rows, R = X.shape[mode], got.shape[1]
+    want = torch.zeros((rows, R), dtype=torch.float64, device=DEV)
+    for s in range(0, X.nnz, 2_000_000):
+        c = coords[:, s:s + 2_000_000]
+        h = [U[m][c[m]].double() for m in range(X.ndim)]
+        model = torch.stack(h).prod(0).sum(1)
+        w = vals[s:s + 2_000_000].double() / model.clamp_min(eps)
+        want.index_add_(0, c[mode], w[:, None] * torch.stack([h[m] for m in range(X.ndim) if m != mode]).prod(0))
+        del h, model, w
+    err = (got.double() - want).abs().amax(1) / want.abs().amax(1).clamp_min(1e-30)
+    worst = float(err.max())
+    del want, err
+    pick = np.sort(np.random.default_rng(seed).choice(rows, sample_rows, replace=False))
+    return {"vs": f"fp64 device evaluation of every row (max |x - x64| / max |x64| <= 1e-4) + {sample_rows} sampled "
+                  "rows bit-compared with the CPU restatement of the order (tests/_cp_apr_order.py)",
+            "values_close": worst <= 1e-4, "worst_row_rel_err": worst,
+            "sampled_rows_bit_exact": CA.sampled_rows_exact(got, coords, vals, U, mode, pick, 512, eps)}
+
+
+def _phi_compare(X, U, mode, eps, card):
+    """The fused call against (a) the two-launch composition on X's cached stream (Kn.tttp of the stream with the
+    values 1, a device clamp and divide, Kn.mttkrp_mode) and (b) the public composed route (tttp on X's pattern, a
+    divide of the data, mttkrp_mode on a new COO, which sorts its own mode stream), timed alternately."""
+    from sparse_b200 import _fused as F
+    from sparse_b200 import _kernels as Kn
+
+    R = U[0].shape[1]
+    coords_s, vals_s = F._mode_stream(X, mode)
+    ones = torch.ones_like(vals_s)
+    rows = X.shape[mode]
+    coords, vals = X._dev()
+    P = sp.COO(coords, torch.ones_like(vals), shape=X.shape, has_duplicates=False, sorted=True)
+
+    def fused():
+        return sp.cp_apr_phi_mode(X, U, mode, eps)
+
+    def two_launch():
+        m = Kn.tttp(coords_s, ones, U, R)
+        return Kn.mttkrp_mode(coords_s, vals_s / torch.where(m < eps, torch.full_like(m, eps), m), U, mode, rows, R)
+
+    def composed():
+        M = sp.tttp(P, U)
+        W = sp.COO(coords, vals / M._dev()[1].clamp_min(eps), shape=X.shape, has_duplicates=False, sorted=True)
+        return sp.mttkrp_mode(W, U, mode)
+
+    out = {"card": card}
+    a, b, c = fused(), two_launch(), composed()
+    out["two_launch_bit_equal_to_fused"] = bool(torch.equal(a.view(torch.int32), b.view(torch.int32)))
+    out["composed_max_rel_diff_vs_fused"] = float(((c.double() - a.double()).abs().amax(1)
+                                                    / a.double().abs().amax(1).clamp_min(1e-30)).max())
+    del a, b, c
+    for name, f in (("fused", fused), ("two_launch", two_launch), ("composed", composed)):
+        torch.cuda.synchronize()
+        torch.cuda.reset_peak_memory_stats(DEV)
+        base = torch.cuda.memory_allocated(DEV)
+        f()
+        torch.cuda.synchronize()
+        out[f"peak_extra_bytes_torch_{name}"] = int(torch.cuda.max_memory_allocated(DEV) - base)
+    ms = _alternate({"fused": fused, "two_launch": two_launch, "composed": composed})
+    out.update({f"ms_median_{k}": v for k, v in ms.items()})
+    out["two_launch_over_fused"] = round(ms["two_launch"] / ms["fused"], 3)
+    out["composed_over_fused"] = round(ms["composed"] / ms["fused"], 3)
+    return out
+
+
+def _cp_apr(rec, parity):
+    """CP-APR's ratio MTTKRP on the CP-ALS workload of mttkrp_mode ((1e6, 1e6, 100), nnz 1e8, f32, values in [0, 1)),
+    nonnegative factors, R = 16 and 32, modes 0 and 2, the mode stream cached; each next to (a) the two-launch
+    composition on the same cached stream and (b) the public composed route; and the same comparison on K9's config
+    (1e4, 1e4, 1e3, nnz 1e7, R = 32)."""
+    sys.path.insert(0, os.path.join(ROOT, "tests"))
+    out = {}
+    card = _card()
+    eps = 1e-10
+    shape = (1_000_000, 1_000_000, 100)
+    X = rand_coo(shape, 100_000_000, 91, torch.float32)
+    for R in (16, 32):
+        g = torch.Generator(device=DEV).manual_seed(95 + R)
+        U = [torch.rand((s, R), generator=g, device=DEV, dtype=torch.float32) for s in shape]
+        for mode in (0, 2):
+            name = f"cp_apr_phi_mode order-3 (1e6,1e6,100) nnz 1e8 R={R} mode {mode} f32"
+            models = _phi_models(X, mode, R)
+            r = rec(name, lambda: sp.cp_apr_phi_mode(X, U, mode, eps), X.nnz, "Gnnz_s", models["bytes"]["total"])
+            r.update(models)
+            r.update(_phi_compare(X, U, mode, eps, card))
+            if parity:
+                got = sp.cp_apr_phi_mode(X, U, mode, eps)
+                r["parity"] = _phi_parity(X, U, mode, eps, got, 8 if mode == 0 else 2, 96)
+                del got
+            out[name] = r
+            print(name, r, flush=True)
+        del U
+    del X
+    torch.cuda.empty_cache()
+
+    X = rand_coo((10_000, 10_000, 1_000), 10_000_000, 31, torch.float32)
+    g = torch.Generator(device=DEV).manual_seed(97)
+    U = [torch.rand((s, 32), generator=g, device=DEV, dtype=torch.float32) for s in X.shape]
+    name = "cp_apr_phi_mode K9 config (1e4,1e4,1e3) nnz 1e7 R=32 mode 0 f32"
+    r = rec(name, lambda: sp.cp_apr_phi_mode(X, U, 0, eps), X.nnz, "Gnnz_s", _phi_models(X, 0, 32)["bytes"]["total"])
+    r.update(_phi_models(X, 0, 32))
+    r.update(_phi_compare(X, U, 0, eps, card))
+    if parity:
+        r["parity"] = _phi_parity(X, U, 0, eps, sp.cp_apr_phi_mode(X, U, 0, eps), 8, 98)
+    out[name] = r
+    print(name, r, flush=True)
+    del X, U
     torch.cuda.empty_cache()
     return out
 

@@ -23,7 +23,8 @@ HOT = [r"spmm_csr_dense_dyn_kernel<float, int, 4, 32, 8, 4>", r"spmm_csr_dense_d
        r"tttp_kernel<double, int, 2>", r"ttm_mode_kernel<float, int, 4>", r"ttm_mode_kernel<float, int, 1>",
        r"ttm_mode_kernel<double, int, 2>", r"cp_completion_kernel<float, int, 4, 4>",
        r"cp_completion_kernel<float, int, 4, 9>", r"cp_completion_kernel<double, int, 2, 9>",
-       r"cp_completion_combine_kernel<float, int>",
+       r"cp_completion_combine_kernel<float, int>", r"cp_apr_phi_kernel<float, int, 4, 4, 4, 4>",
+       r"cp_apr_phi_kernel<float, int, 4, 8, 4, 4>", r"cp_apr_phi_kernel<double, int, 2, 32, 2, 8>",
        r"masked_spgemm_kernel<float, float, int, 32>", r"masked_spgemm_kernel<double, double, int, 8>",
        r"spmm_bulk_kernel<float"]
 
