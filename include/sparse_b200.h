@@ -469,6 +469,31 @@ int b2s_ttm_mode(int dtype, int idx_bytes, int64_t n_fibers, int64_t R, int64_t 
 int b2s_ttm_mode_long_flags(int idx_bytes, int64_t n_fibers, const void *fptr_dev, int64_t long_min,
                             uint8_t *flags_out_dev, void *stream);
 
+/* ---- sparse x sparse tensor contraction with a sparse result (K17, sptc.cu; the sums are K4's) ---------------------
+ * sptc(X, Y, axes) contracts the paired axes of two sparse tensors of order 1..8.  With F / C the C-order linear keys
+ * of an X entry over its free / contracted axes (contracted axes in the order `axes` pairs them), and C / G the same
+ * for a Y entry: for every (F, G) that has at least one common C,
+ *     z(F, G) = ((+0 + x(F, C_1) * y(C_1, G)) + x(F, C_2) * y(C_2, G)) + ...    over the common C, ascending,
+ * each product and sum rounded in the result dtype (no FMA; integers wrap).  z is stored iff bits(z) != bits(+0), so
+ * -0.0 and NaN stay; its key is F * G_ext + G (G_ext the product of Y's free extents), and the keys ascend.  This is
+ * b2s_spgemm's SORTED order with prune on the matricised operands, so wherever tensordot fits the result equals
+ * tensordot(X, Y, axes, return_type=COO) bit for bit.
+ *
+ * The operands are doubly-compressed CSR: xrows[nF] / yrows[nC] list the distinct row keys, ascending, with pointer
+ * arrays of nF + 1 / nC + 2 entries (Y has one more, empty, row nC), and Y's columns are ranks among its distinct free
+ * keys ycols[nG].  b2s_spgemm runs on (nF x (nC + 1)) @ ((nC + 1) x nG); the two entries below are the steps around it.
+ * Neither synchronises the stream, uses atomics or allocates.
+ *
+ * b2s_sptc_join: out[q] = the index of query[q] in set[0..ns) (int64, ascending, no duplicates), or ns when it is not
+ * there; out is idx_bytes wide (4 needs ns < 2^31 - 1).  Any query order is allowed.  query_dev and out_dev must be
+ * 16-byte aligned. */
+int b2s_sptc_join(int idx_bytes, int64_t nq, const int64_t *query_dev, int64_t ns, const int64_t *set_dev,
+                  void *out_dev, void *stream);
+/* b2s_sptc_keys: keys_out[i] = xrows[rows[i]] * g_ext + ycols[cols[i]], i < n, for b2s_spgemm's (rows, cols) output;
+ * the caller has checked that the products fit int64.  rows_dev, cols_dev and keys_out_dev must be 16-byte aligned. */
+int b2s_sptc_keys(int64_t n, const int64_t *rows_dev, const int64_t *cols_dev, const int64_t *xrows_dev,
+                  const int64_t *ycols_dev, int64_t g_ext, int64_t *keys_out_dev, void *stream);
+
 /* ---- masked sparse x sparse product (K11, masked_spgemm.cu; examples/triangles_example.py) ------------------------
  * out_vals[p] = value of mask * (A @ B) at every stored mask entry p, given the mask as CSR (m_indptr over the M rows,
  * m_cols, m_vals already in the output dtype `dtype_out`), A as CSR (M x K) and B^T as CSR (N x K, i.e. B by

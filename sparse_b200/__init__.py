@@ -39,7 +39,7 @@ from ._dok import DOK
 from ._dot import dot, matmul, tensordot
 from ._einsum import einsum
 from ._elemwise import broadcast_to, elemwise, where
-from ._fused import (cp_apr_phi_mode, cp_completion_mode, masked_matmul, mttkrp, mttkrp_mode, sddmm, ttm_mode,
+from ._fused import (cp_apr_phi_mode, cp_completion_mode, masked_matmul, mttkrp, mttkrp_mode, sddmm, sptc, ttm_mode,
                      ttmc_mode, tttp)
 from ._gcxs import CSC, CSR, GCXS
 from ._io import load_npz, save_npz
@@ -52,7 +52,7 @@ from ._sparse_array import SparseArray
 
 __version__ = "0.1.0"
 # `__all__` below is exactly upstream's namespace (tests/test_namespace.py there); the fused kernels `sddmm`, `mttkrp`,
-# `mttkrp_mode`, `ttmc_mode`, `tttp`, `ttm_mode`, `cp_completion_mode`, `cp_apr_phi_mode` and `masked_matmul`, the 2-D classes `CSR` / `CSC` and a few helpers are importable attributes outside of it.
+# `mttkrp_mode`, `ttmc_mode`, `tttp`, `ttm_mode`, `sptc`, `cp_completion_mode`, `cp_apr_phi_mode` and `masked_matmul`, the 2-D classes `CSR` / `CSC` and a few helpers are importable attributes outside of it.
 
 
 def clip(a, min=None, max=None, out=None):

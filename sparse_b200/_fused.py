@@ -16,6 +16,8 @@ ttm_mode(X, U, mode) is the mode-n tensor times matrix (or vector) with a sparse
 cp_completion_mode(X, factors, mode, reg) is the row-wise least-squares ALS update of CP completion, and
 cp_apr_phi_mode(X, factors, mode, eps) the ratio MTTKRP of Poisson CP (CP-APR): mttkrp_mode of X / max(model, eps)
 at X's entries, fused on the same cached mode stream.
+sptc(X, Y, axes) is tensordot for two sparse tensors with a sparse result, bit for bit, on rows that exist only where
+there are entries: its memory does not depend on the extents.
 
 masked_matmul(mask, a, b) == mask * (a @ b) at mask's stored positions, for sparse a and b: the masked SpGEMM of
 examples/triangles_example.py (sum(a @ a * a) / 6) and of the GraphBLAS masked mxm.  It never forms the product
@@ -565,6 +567,150 @@ def ttm_mode(X, U, mode):
 _FORCE_WIDE_INDEX_MASKED = False
 
 _MASKED_DTYPES = tuple(np.dtype(d) for d in ("float32", "float64", "int32", "int64"))
+
+# Test hook: True keeps sptc's index arrays int64 even when every row count and nnz fit int32.
+_FORCE_WIDE_INDEX_SPTC = False
+
+
+def _sptc_axes(X, Y, axes):
+    """The contracted axes of X and of Y as two lists of non-negative ints, paired in order: the `axes` forms, checks
+    and errors of `tensordot`."""
+    try:
+        iter(axes)
+    except TypeError:
+        axes_x, axes_y = list(range(-axes, 0)), list(range(axes))
+    else:
+        axes_x, axes_y = axes
+    axes_x = list(axes_x) if hasattr(axes_x, "__len__") else [axes_x]
+    axes_y = list(axes_y) if hasattr(axes_y, "__len__") else [axes_y]
+    if X.ndim == 0 or Y.ndim == 0:
+        raise ValueError(f"Input {int(X.ndim != 0)} operand does not have enough dimensions")
+    equal = len(axes_x) == len(axes_y)
+    for k in range(len(axes_x) if equal else 0):
+        if X.shape[axes_x[k]] != Y.shape[axes_y[k]]:
+            equal = False
+            break
+        axes_x[k] %= X.ndim
+        axes_y[k] %= Y.ndim
+    if not equal or len(set(axes_x)) != len(axes_x) or len(set(axes_y)) != len(axes_y):
+        raise ValueError("shape-mismatch for sum")
+    return axes_x, axes_y
+
+
+def _sptc_stream(X, free, con, side, narrow):
+    """One operand of sptc as doubly-compressed CSR, cached on X under ("sptc", side, contracted axes, int32 indices)
+    and dropped with the other streams.  The entries are ordered by the key over (free axes, contracted axes) for side
+    "x" and (contracted axes, free axes) for side "y": X's canonical order when that is its axis order, one stable sort
+    otherwise.  Rows exist only where there are entries.
+
+    "x": (row keys F [nF] int64, row pointers [nF + 1], contracted key C of every entry [nnz] int64, values)
+    "y": (row keys C [nC] int64, row pointers [nC + 2] with an empty last row, distinct free keys G [nG] int64,
+          the rank of every entry's G among them [nnz], values)"""
+    from ._gcxs import GCXS
+    from ._utils import key_bits, prod
+
+    key = ("sptc", side, tuple(con), narrow)
+    cache = X._mode_streams
+    if cache is not None and key in cache:
+        return cache[key]
+    c = X.tocoo() if isinstance(X, GCXS) else X
+    order = list(free) + list(con) if side == "x" else list(con) + list(free)
+    inner = prod(X.shape[a] for a in (con if side == "x" else free))
+    keys, data = c._permuted_keys(order)
+    nnz = X.nnz
+    rows, cols, _ = Kn.csr_from_keys(keys, 0, inner, np.int64, want_rows=True, want_indptr=False)
+    heads = Kn.flag_heads(rows)
+    pos, nr = Kn.scan_flags(heads)
+    rowkeys = Kn.compact(rows, heads, pos, nr)
+    t = D.torch()
+    ptr = t.cat([Kn.compact(Kn.iota(nnz), heads, pos, nr), Kn.full(1 if side == "x" else 2, nnz, np.int64)])
+    idt = np.int32 if narrow else np.int64
+    ptr = Kn.cast(ptr, idt)
+    if side == "x":
+        stream = (rowkeys, ptr, cols, data)
+    else:
+        by_col, _ = Kn.sort_keys(cols, key_bits(inner))
+        cheads = Kn.flag_heads(by_col)
+        cpos, ng = Kn.scan_flags(cheads)
+        colkeys = Kn.compact(by_col, cheads, cpos, ng)
+        stream = (rowkeys, ptr, colkeys, Kn.sptc_join(cols, colkeys, idt), data)
+    if cache is None:
+        cache = X._mode_streams = {}
+    cache[key] = stream
+    return stream
+
+
+def sptc(X, Y, axes=2):
+    """Sparse x sparse tensor contraction with a sparse result: ``tensordot(X, Y, axes)`` for two sparse tensors whose
+    extents are far larger than their numbers of entries -- contracting two sparse tensors of a tensor network or a
+    quantum-chemistry code, chaining sparse Tucker cores, a TTM with a sparse matrix.
+
+        Z[f_1, ..., g_1, ...] = sum over the contracted index tuples c of  X[f..., c...] * Y[c..., g...]
+
+    `X` and `Y` are COO or GCXS arrays of order 1..8 with a zero fill value (a GCXS computes as its ``tocoo()``).
+    `axes` has tensordot's forms: an int n (the last n axes of X with the first n of Y) or ``(axes_x, axes_y)``, ints
+    or sequences, negative axes counting from the end, paired in the order given.  The dtype is that of ``X * Y``:
+    float32, float64, int32 or int64, and int8 / int16 / uint8 / uint16 / uint32 through a wider integer as in
+    tensordot; anything else raises TypeError.  The result is always a canonical COO of shape free(X) + free(Y) with
+    fill value +0.  A dense or GCXS result is not offered: it would span the extents this op leaves out.
+
+    The order of operations is fixed (include/sparse_b200.h, b2s_sptc_join): each value is ((+0 + x_1 * y_1) +
+    x_2 * y_2) + ... over the common contracted indices in ascending C order, each product and sum rounded, integers
+    wrapping, and a value is stored iff its bits differ from +0 (-0.0 and NaN stay).  Wherever tensordot fits in
+    memory, ``sptc(X, Y, axes)`` equals ``tensordot(X.tocoo(), Y.tocoo(), axes, return_type=COO)`` bit for bit.
+    tensordot builds a row pointer over the product of X's free extents and another over the product of the contracted
+    extents; sptc keeps only the rows that hold entries, so its memory is O(nnz(X) + nnz(Y) + products) whatever the
+    extents.  The products of X's and Y's free extents together, and of the contracted extents, must be below 2**63
+    (ValueError before anything is allocated).
+
+    Memory: each operand's compressed rows are cached on it for the next call with the same side and contracted axes
+    (dropped when its contents are replaced, not copied or pickled).  X holds nnz * (8 + value bytes) + nF * (8 + index
+    bytes), Y nnz * (index bytes + value bytes) + nC * (8 + index bytes) + nG * 8, with nF / nC / nG the numbers of
+    distinct free keys of X, contracted keys of Y and free keys of Y, and index bytes 4 when both nnz fit int32, else
+    8; the values are X's own array when no sort was needed.  During the call: nnz(X) * index bytes for the join, K4's
+    scratch (proportional to nF and to the products) and the result, nnz(Z) * (value bytes + 8) plus 16 bytes per entry
+    of K4's row and column output.
+    """
+    from ._dot import _dot_dtype
+    from ._elemwise import _WIDE_FOR
+    from ._gcxs import GCXS
+    from ._utils import prod
+
+    for name, x in (("X", X), ("Y", Y)):
+        if not isinstance(x, (COO, GCXS)):
+            raise TypeError(f"sptc: `{name}` must be a sparse_b200 COO or GCXS array")
+    check_zero_fill_value(X, Y)
+    axes_x, axes_y = _sptc_axes(X, Y, axes)
+    for name, x in (("X", X), ("Y", Y)):
+        if x.ndim > 8:
+            raise ValueError(f"sptc: order {x.ndim} of `{name}` outside 1..8")
+    T = _dot_dtype(X.dtype, Y.dtype)
+    Tc = _WIDE_FOR.get(T, T)
+    if Tc not in _MASKED_DTYPES:
+        raise TypeError(f"sptc: dtypes ({X.dtype}, {Y.dtype}) are outside the CUDA dtype matrix (float32, float64, "
+                        "int32, int64, and the narrower integers through them)")
+    free_x = [a for a in range(X.ndim) if a not in axes_x]
+    free_y = [a for a in range(Y.ndim) if a not in axes_y]
+    shape = tuple(X.shape[a] for a in free_x) + tuple(Y.shape[a] for a in free_y)
+    g_ext = prod(Y.shape[a] for a in free_y)
+    if prod(shape) >= 2**63:
+        raise ValueError(f"sptc: result shape {shape} has 2**63 elements or more (the COO index limit)")
+    if prod(X.shape[a] for a in axes_x) >= 2**63:
+        raise ValueError(f"sptc: the contracted extents {tuple(X.shape[a] for a in axes_x)} have a product of 2**63 or "
+                         "more")
+    if X.nnz == 0 or Y.nnz == 0:
+        return COO._from_device(None, Kn.full(0, 0, T), shape, T.type(0), keys=Kn.full(0, 0, np.int64))
+    narrow = not _FORCE_WIDE_INDEX_SPTC and max(X.nnz, Y.nnz) + 1 < 2**31 - 1
+    xrows, xptr, xcon, xvals = _sptc_stream(X, free_x, axes_x, "x", narrow)
+    yrows, yptr, ycols, yrank, yvals = _sptc_stream(Y, free_y, axes_y, "y", narrow)
+    nC = int(yrows.shape[0])
+    # an X entry whose contracted key no Y entry has gets column nC, Y's empty last row: X needs no compaction
+    joined = Kn.sptc_join(xcon, yrows, np.int32 if narrow else np.int64)
+    _, cols, rows, data, _ = Kn.spgemm(xptr, joined, Kn.cast(xvals, Tc), yptr, yrank, Kn.cast(yvals, Tc),
+                                       int(xrows.shape[0]), nC + 1, int(ycols.shape[0]), sorted_order=True, prune=True,
+                                       want_indptr=False, want_rows=True)
+    res = COO._from_device(None, data, shape, Tc.type(0), keys=Kn.sptc_keys(rows, cols, xrows, ycols, g_ext))
+    return res if Tc == T else res.astype(T, _raw=True)
 
 
 def _rows_of_b(b, Tc):

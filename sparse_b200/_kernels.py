@@ -818,6 +818,28 @@ def ttm_mode(kcoord, vals, fptr, fgroup, gptr, fkey, pkey, long_ids, long_min, U
 
 
 # ------------------------------------------------------------------------------------------------
+# K17 sparse x sparse tensor contraction: the join and the result keys around K4
+# ------------------------------------------------------------------------------------------------
+def sptc_join(query, keys, idx_dtype=np.int64):
+    """out[q] = the index of query[q] in the ascending, duplicate-free int64 array `keys`, or len(keys) when it is not
+    there (b2s_sptc_join); `query` is int64 in any order, the result has `idx_dtype` (int32 / int64)."""
+    t = _t()
+    out = t.empty(query.shape[0], dtype=D.torch_dtype(idx_dtype), device=query.device)
+    _lib.check(_lib.load().b2s_sptc_join(i32(np.dtype(idx_dtype).itemsize), i64(query.shape[0]), vp(D.ptr(query)),
+                                         i64(keys.shape[0]), vp(D.ptr(keys)), vp(D.ptr(out)), _sp()), "b2s_sptc_join")
+    return out
+
+
+def sptc_keys(rows, cols, xrows, ycols, g_ext):
+    """keys[i] = xrows[rows[i]] * g_ext + ycols[cols[i]] for K4's int64 (rows, cols) output (b2s_sptc_keys)."""
+    t = _t()
+    keys = t.empty(rows.shape[0], dtype=t.int64, device=rows.device)
+    _lib.check(_lib.load().b2s_sptc_keys(i64(rows.shape[0]), vp(D.ptr(rows)), vp(D.ptr(cols)), vp(D.ptr(xrows)),
+                                         vp(D.ptr(ycols)), i64(g_ext), vp(D.ptr(keys)), _sp()), "b2s_sptc_keys")
+    return keys
+
+
+# ------------------------------------------------------------------------------------------------
 # K11 masked SpGEMM
 # ------------------------------------------------------------------------------------------------
 def masked_spgemm(m_indptr, m_cols, m_vals, a_indptr, a_cols, a_vals, bt_indptr, bt_cols, bt_vals, M, N, K):

@@ -5,11 +5,12 @@ Device-resident inputs (generated with seeded torch generators on the GPU), wall
 torch.cuda.synchronize() because the public calls contain their own size-returning syncs.
 Prints one line per config as it runs and the whole result as one JSON line at the end.
 
-    python tools/bench_configs.py [c1 c3 c3big red c4 c5 mttkrp mttkrp_mode masked ttmc tttp ttm completion cp_apr]
+    python tools/bench_configs.py [c1 c3 c3big red c4 c5 mttkrp mttkrp_mode masked ttmc tttp ttm completion cp_apr sptc]
 
 `masked` (the masked SpGEMM, examples/triangles_example.py), `ttmc` (the Tucker / HOOI step), `tttp` (a CP model at
 a sparse tensor's entries), `ttm` (mode-n tensor times matrix with a sparse result), `completion` (the ALS update
-of CP tensor completion) and `cp_apr` (the ratio MTTKRP of Poisson CP) run only when named.
+of CP tensor completion), `cp_apr` (the ratio MTTKRP of Poisson CP) and `sptc` (sparse x sparse tensor contraction on
+compressed rows) run only when named.
 """
 import json
 import os
@@ -290,6 +291,8 @@ def run(which=None, compact=False, parity=True):
         res.update(_completion(rec, parity))
     if "cp_apr" in which:
         res.update(_cp_apr(rec, parity))
+    if "sptc" in which:
+        res.update(_sptc(rec, parity))
     torch.cuda.empty_cache()
     return res
 
@@ -1180,6 +1183,156 @@ def _cp_apr(rec, parity):
     out[name] = r
     print(name, r, flush=True)
     del X, U
+    torch.cuda.empty_cache()
+    return out
+
+
+def _sptc_fp64(X, Y, ax, ay):
+    """(keys, values) of the contraction in float64 on the device: every X entry joined with the Y entries of its
+    contracted key (searchsorted + repeat_interleave), the products summed per result key with index_add_."""
+    free_x = [a for a in range(X.ndim) if a not in ax]
+    free_y = [a for a in range(Y.ndim) if a not in ay]
+
+    def key(c, shape, axes):
+        k = torch.zeros(c.shape[1], dtype=torch.int64, device=DEV)
+        for a in axes:
+            k = k * shape[a] + c[a]
+        return k
+
+    xc, xv = X._dev()
+    yc, yv = Y._dev()
+    g_ext = int(np.prod([Y.shape[a] for a in free_y], dtype=object))
+    yC, order = torch.sort(key(yc, Y.shape, ay), stable=True)
+    yG, yv = key(yc, Y.shape, free_y)[order], yv[order].double()
+    xC, xF = key(xc, X.shape, ax), key(xc, X.shape, free_x)
+    lo, hi = torch.searchsorted(yC, xC), torch.searchsorted(yC, xC, right=True)
+    cnt = hi - lo
+    src = torch.repeat_interleave(torch.arange(xC.numel(), device=DEV), cnt)
+    off = torch.arange(src.numel(), device=DEV) - torch.repeat_interleave(torch.cumsum(cnt, 0) - cnt, cnt)
+    tgt = lo[src] + off
+    keys, inv = torch.unique(xF[src] * g_ext + yG[tgt], return_inverse=True)
+    vals = torch.zeros(keys.numel(), dtype=torch.float64, device=DEV).index_add_(0, inv, xv.double()[src] * yv[tgt])
+    return keys, vals, int(src.numel())
+
+
+def _sptc_parity(X, Y, ax, ay, got, sample_rows, seed):
+    """Every value against the fp64 device restatement, and `sample_rows` result rows (free keys of X) bit-compared with
+    the CPU restatement of the contract (tests/_sptc_order.py)."""
+    import _sptc_order as SO
+
+    keys, vals, products = _sptc_fp64(X, Y, ax, ay)
+    gk, gv = got.sorted_keys(), got._data_dev()
+    pos = torch.searchsorted(keys, gk).clamp_(max=max(keys.numel() - 1, 0))
+    present = bool((keys[pos] == gk).all())
+    w = vals[pos]
+    close = present and bool(torch.allclose(gv.double(), w, rtol=2e-5, atol=2e-5 * float(w.abs().max())))
+    free_y = [a for a in range(Y.ndim) if a not in ay]
+    g_ext = int(np.prod([Y.shape[a] for a in free_y], dtype=object))
+    rows = torch.unique(torch.div(gk, g_ext, rounding_mode="floor"))
+    rng = np.random.default_rng(seed)
+    pick = rows[torch.from_numpy(np.sort(rng.choice(rows.numel(), min(sample_rows, rows.numel()), replace=False))).to(DEV)]
+    xc, xv = X._dev()
+    free_x = [a for a in range(X.ndim) if a not in ax]
+    xF = torch.zeros(X.nnz, dtype=torch.int64, device=DEV)
+    for a in free_x:
+        xF = xF * X.shape[a] + xc[a]
+    xsel = torch.isin(xF, pick)
+    xC = torch.zeros(X.nnz, dtype=torch.int64, device=DEV)
+    for a in ax:
+        xC = xC * X.shape[a] + xc[a]
+    yc, yv = Y._dev()
+    yC = torch.zeros(Y.nnz, dtype=torch.int64, device=DEV)
+    for a in ay:
+        yC = yC * Y.shape[a] + yc[a]
+    ysel = torch.isin(yC, torch.unique(xC[xsel]))
+    rk, rv = SO.result(xc[:, xsel].cpu().numpy(), xv[xsel].cpu().numpy(), X.shape, yc[:, ysel].cpu().numpy(),
+                       yv[ysel].cpu().numpy(), Y.shape, ax, ay, got.dtype)
+    gsel = torch.isin(torch.div(gk, g_ext, rounding_mode="floor"), pick)
+    exact = bool(np.array_equal(gk[gsel].cpu().numpy(), rk) and SO.same_bits(gv[gsel].cpu().numpy(), rv))
+    return {"vs": "fp64 device restatement (rtol 2e-5 of the largest value) and sampled result rows bit-compared with "
+                  "tests/_sptc_order.py", "values_close": close, "sampled_rows": int(pick.numel()),
+            "sampled_rows_bit_exact": exact}, products
+
+
+def _sptc_stages(X, Y, ax, ay):
+    """ms of the stages of one cached call, each between device synchronisations: the join, K4, the result keys."""
+    from sparse_b200 import _fused as F
+    from sparse_b200 import _kernels as Kn
+
+    free_x = [a for a in range(X.ndim) if a not in ax]
+    free_y = [a for a in range(Y.ndim) if a not in ay]
+    xrows, xptr, xcon, xvals = F._sptc_stream(X, free_x, ax, "x", True)
+    yrows, yptr, ycols, yrank, yvals = F._sptc_stream(Y, free_y, ay, "y", True)
+    g_ext = int(np.prod([Y.shape[a] for a in free_y], dtype=object))
+    nF, nC, nG = int(xrows.shape[0]), int(yrows.shape[0]), int(ycols.shape[0])
+    joined = Kn.sptc_join(xcon, yrows, np.int32)
+    k4 = lambda: Kn.spgemm(xptr, joined, xvals, yptr, yrank, yvals, nF, nC + 1, nG, sorted_order=True, prune=True,
+                           want_indptr=False, want_rows=True)
+    _, cols, rows, _, _ = k4()
+    t = _alternate({"join": lambda: Kn.sptc_join(xcon, yrows, np.int32), "k4": k4,
+                    "keys": lambda: Kn.sptc_keys(rows, cols, xrows, ycols, g_ext)})
+    return {"stage_ms_median": t, "nF": nF, "nC": nC, "nG": nG}
+
+
+def _sptc(rec, parity):
+    """Sparse x sparse tensor contraction.  Where tensordot fits, sptc and tensordot(return_type=COO) alternating with
+    both calls' peak extra device memory and a bit comparison; a hypersparse pair that tensordot cannot take, with the
+    first call (stream build), the cached call, its stages and the byte model of the two new kernels."""
+    sys.path.insert(0, os.path.join(ROOT, "tests"))
+    out = {}
+    card = _card()
+
+    X = rand_coo((10_000, 1_000, 1_000), 10_000_000, 101, torch.float32)
+    Y = rand_coo((1_000, 1_000, 64), 1_000_000, 102, torch.float32)
+    ax, ay = [1, 2], [0, 1]
+    fns = {"sptc": lambda: sp.sptc(X, Y, (ax, ay)), "tensordot": lambda: sp.tensordot(X, Y, (ax, ay), return_type=sp.COO)}
+    peak = {}
+    for k, fn in fns.items():
+        fn()
+        torch.cuda.synchronize()
+        torch.cuda.reset_peak_memory_stats(DEV)
+        base = torch.cuda.memory_allocated(DEV)
+        fn()
+        torch.cuda.synchronize()
+        peak[k] = int(torch.cuda.max_memory_allocated(DEV) - base)
+    t = _alternate(fns)
+    got, want = fns["sptc"](), fns["tensordot"]()
+    name = "sptc (1e4,1e3,1e3) nnz 1e7 . (1e3,1e3,64) nnz 1e6 over two modes f32 vs tensordot(return_type=COO)"
+    r = {"ms_median": t["sptc"], "tensordot_ms_median": t["tensordot"],
+         "speedup_vs_tensordot": round(t["tensordot"] / t["sptc"], 2), "peak_extra_bytes_streams_cached": peak["sptc"],
+         "tensordot_peak_extra_bytes": peak["tensordot"], "out_nnz": got.nnz, "card": card,
+         **_sptc_stages(X, Y, ax, ay),
+         "whole_result_bit_exact_vs_tensordot": bool(
+             got.nnz == want.nnz and torch.equal(got.sorted_keys(), want.sorted_keys())
+             and torch.equal(got._data_dev().view(torch.int32), want._data_dev().view(torch.int32)))}
+    print(name, r, flush=True)
+    out[name] = r
+    del X, Y, got, want
+    torch.cuda.empty_cache()
+
+    # hypersparse: the matricised X has 1e12 rows and the contracted extent is 1e6; sizes chosen so that the result
+    # (about two products per X entry) stays near 4e7 entries
+    X = rand_coo((1_000_000,) * 3, 20_000_000, 103, torch.float32)
+    Y = rand_coo((1_000_000, 100_000), 2_000_000, 104, torch.float32)
+    ax, ay = [2], [0]
+    torch.cuda.synchronize()
+    t0 = time.perf_counter()
+    got = sp.sptc(X, Y, (ax, ay))
+    torch.cuda.synchronize()
+    first = (time.perf_counter() - t0) * 1e3
+    name = "sptc hypersparse (1e6,1e6,1e6) nnz 2e7 . (1e6,1e5) nnz 2e6 over the last mode f32"
+    r = rec(name, lambda: sp.sptc(X, Y, (ax, ay)), X.nnz, "Gnnz_s")
+    st = _sptc_stages(X, Y, ax, ay)
+    model = {"join_bytes": X.nnz * (8 + 4) + st["nC"] * 8, "keys_bytes": got.nnz * (16 + 8)}
+    r.update({"card": card, "first_call_ms_incl_streams": round(first, 3), "out_nnz": got.nnz, **st,
+              "model_bytes": model,
+              "model_join_GBs": round(model["join_bytes"] / st["stage_ms_median"]["join"] / 1e6, 1),
+              "model_keys_GBs": round(model["keys_bytes"] / st["stage_ms_median"]["keys"] / 1e6, 1)})
+    if parity:
+        r["parity"], r["products"] = _sptc_parity(X, Y, ax, ay, got, 2_000, 105)
+    print(name, r, flush=True)
+    out[name] = r
+    del X, Y, got
     torch.cuda.empty_cache()
     return out
 
